@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
-"""bench.py — decode tokens/s of the GGUF-quantised hot path on B200 (BASELINE.json metric).
+"""bench.py — decode tokens/s of the GGUF-quantised hot path on H100 (BASELINE.json metric).
 
 A "step" is one batch-1 decode token of Llama-3-8B Q4_K_M (synthetic random-valid GGUF blocks of that
 architecture — no weights ship with the reference and there is no network): the full node list libllama
 emits for one token (32 layers + lm_head, 7 quantised matvecs / layer, rms_norm, rope, KV store,
-flash-attention over an F16 KV cache), run on hand-written sm_100a kernels.
+flash-attention over an F16 KV cache), run on hand-written sm_90a kernels.
 
 N = 1
   value        : tokens/s with every input resident in HBM (graph executor C-ABI, token feedback through an on-device argmax)
@@ -17,10 +17,13 @@ N = 1
                  replayed as a CUDA graph; algorithmic weight bytes / CUDA-event time, against MEASURED_PEAKS.json
   cpu_baseline : the reference's own ggml-cpu path (oracle/_ref: unmodified libllama + libggml-cpu built from
                  /root/reference) on the box's host cores, same architecture / quant mix
-  gpu_reference: (informational) the reference's own ggml-cuda backend (oracle/_ref_cuda, built unmodified for sm_100) on the
+  gpu_reference: (informational) the reference's own ggml-cuda backend (oracle/_ref_cuda, built unmodified for sm_90) on the
                  same GGUF through the same driver — the GPU bar to beat
   depth, prefill: (informational) the same metric at n_past ~3800, and prefill tok/s (config 3) through the product path
   --impl reference : the CPU path as its own arm (3 repeats, threads = CPUs this process may run on)
+  --dump-outputs DIR: after the timed steps, what the last timed step handed its caller — logits.npy (f32 [n_vocab]) and
+                 token.npy (the on-device argmax, f64 [1]) — so that two builds can be compared output for output; weights
+                 (model.py seed), KV-cache contents and positions are seeded, so the same arguments give the same inputs
 
 N > 1 (torchrun): the reference's LLAMA_SPLIT_MODE_LAYER through the product boundary: ONE process (rank 0) drives all N devices
 with --tensor-split 1,..,1 at true batch 1 (libllama's scheduler hands the hidden state from device to device through the
@@ -63,12 +66,17 @@ def parse():
     ap.add_argument("--no-fusion", action="store_true")
     ap.add_argument("--mega", action="store_true", help="experimental: attention as a phase of the persistent decode kernel")
     ap.add_argument("--mega-mmv", action="store_true", help="experimental: attention and the matvecs inside the persistent decode kernel")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's logits / token as DIR/<name>.npy (single-GPU device-resident leg only)")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.gpus > 1 or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        ap.error("--dump-outputs writes what the single-GPU device-resident leg computed: not with --impl reference or more than one GPU")
+    return args
 
 
 # ------------------------------------------------------------------------------------------------ clocks
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)"""
 
     def __init__(self, gpu_index=0):
         self.proc, self.lines, self.gpu, self.t_begin = None, [], gpu_index, None
@@ -121,7 +129,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 def kernel_traffic():
@@ -320,7 +328,7 @@ def run_b200(args):
     stream = torch.cuda.Stream()
     hbm_peak, peak_src = peaks()
 
-    res = device_resident_leg(args, model, ex, ops, G, stream, flags, args.n_past, args.steps, args.warmup, local, clocks=True)
+    res = device_resident_leg(args, model, ex, ops, G, stream, flags, args.n_past, args.steps, args.warmup, local, clocks=True, dump=args.dump_outputs)
     tps, ms_per_step = res["tps"], res["ms_per_step"]
 
     # ---- roofline leg: the matvec launches of the step, in situ
@@ -371,7 +379,7 @@ def run_b200(args):
     if not args.no_extras and os.path.exists(REF_CUDA):
         o = drv_subprocess(args, REF_CUDA, 99, min(args.n_past, 512), 65, timeout=600)
         if o and "error" not in o:
-            gpu_ref = {"decode_tok_s": o["decode_tps"], "prefill_tok_s": o["prefill_tps"], "backend": "ggml-cuda, unmodified, sm_100 build (oracle/_ref_cuda), CUDA graphs on, -fa",
+            gpu_ref = {"decode_tok_s": o["decode_tps"], "prefill_tok_s": o["prefill_tps"], "backend": "ggml-cuda, unmodified, sm_90 build (oracle/_ref_cuda), CUDA graphs on, -fa",
                        "sample": "64 greedy tokens after a %d-token prompt, wall clock of llama_drv" % o["prompt_len"]}
             o2 = drv_subprocess(args, REF_CUDA, 99, 4096, 2, timeout=600)
             if o2 and "error" not in o2:
@@ -396,15 +404,16 @@ def run_b200(args):
 def whole_step(model, res, hbm_peak):
     b = res["weight_bytes"] + res["n_kv_mid"] * res["kv_bytes_per_pos"] + res["kv_bytes_per_pos"]
     ach = b / (res["ms_per_step"] * 1e-3) / 1e9
-    return {"bytes": b, "achieved": ach, "unit": "GB/s", "frac": ach / hbm_peak, "frac_of_8TBs": ach / 8000.0}
+    return {"bytes": b, "achieved": ach, "unit": "GB/s", "frac": ach / hbm_peak, "frac_of_3_35TBs": ach / 3350.0}
 
 
 def n_kv_of(pos):
     return max(256, (pos + 1 + 255) // 256 * 256)
 
 
-def device_resident_leg(args, model, ex, ops, G, stream, flags, n_past, steps, warmup, local, clocks):
-    """`value`: every input already in HBM — 3 tiny D2D copies + the token graph + on-device argmax feeding the next step"""
+def device_resident_leg(args, model, ex, ops, G, stream, flags, n_past, steps, warmup, local, clocks, dump=None):
+    """`value`: every input already in HBM — 3 tiny D2D copies + the token graph + on-device argmax feeding the next step.
+    `dump`: directory that receives the last timed step's logits and sampled token (.npy), written after the timing"""
     import torch
     c = model.c
     V = c["n_vocab"]
@@ -467,6 +476,12 @@ def device_resident_leg(args, model, ex, ops, G, stream, flags, n_past, steps, w
         launches = ops.lib.b200_kernel_launches() - l0
         ms = e0.elapsed_time(e1)
         clk = sampler.stop() if sampler else None
+    if dump:
+        import numpy as np
+        _, io = nodes_for(n_kv_of(n_past + total - 1))
+        os.makedirs(dump, exist_ok=True)
+        np.save(os.path.join(dump, "logits.npy"), io["logits"][0].float().cpu().numpy())
+        np.save(os.path.join(dump, "token.npy"), io["tokens"][:1].cpu().numpy().astype(np.float64))
     ms_per_step = ms / steps
     return {"tps": 1000.0 / ms_per_step, "ms_per_step": ms_per_step, "launches": launches, "kernels_per_step": ex.last_kernels + 1, "clocks": clk,
             "weight_bytes": model.streamed_weight_bytes(), "kv_bytes_per_pos": model.kv_bytes_per_pos(), "n_kv_mid": n_kv_of(n_past + warmup + steps // 2), "n_layer": len(model.layers)}
@@ -501,7 +516,7 @@ def mmvq_roofline_insitu(args, model, ex, ops, G, stream, flags, hbm_peak):
     if kt and "mmvq_per_token_dram_bytes" in kt:
         traffic, src = int(kt["mmvq_per_token_dram_bytes"]), kt.get("source", "profiles/r2_kernel_traffic.json")
     return {"bound": "hbm", "kernel": "quantised matvec launches of one token, in situ (mmvq_kernel + the lm_head launch; %d kernels incl. the embedding gather)" % nl,
-            "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "frac_of_8TBs": ach / 8000.0, "traffic": traffic, "traffic_source": src,
+            "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "frac_of_3_35TBs": ach / 3350.0, "traffic": traffic, "traffic_source": src,
             "bytes_per_token": wbytes, "launches_per_token": int(nl), "avg_launch_us": ms * 1e3 / max(1, nl), "ms_per_token_matvec_only": ms}
 
 

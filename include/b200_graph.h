@@ -9,7 +9,7 @@
  * capture of ggml-cuda (ggml/src/ggml-cuda/ggml-cuda.cu:2845-3010, 2784-2843, 2593-2782).
  *
  * What the executor does with a node list:
- *   - skips view ops, launches one hand-written sm_100a kernel per remaining node, or fewer:
+ *   - skips view ops, launches one hand-written sm_90a kernel per remaining node, or fewer:
  *       RMS_NORM+MUL(+activation quantisation), MUL_MAT+ADD(bias)+ADD(residual),
  *       MUL_MAT(up)+MUL_MAT(gate)+GLU, several MUL_MATs of one activation in one launch (QKV),
  *   - quantises each activation tensor once per consumer group (the reference re-quantises per matmul),

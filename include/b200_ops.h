@@ -1,5 +1,5 @@
 /*
- * b200_ops.h — C-ABI of libb200ops.so: the hand-written sm_100a kernels for the GGUF-quantized
+ * b200_ops.h — C-ABI of libb200ops.so: the hand-written sm_90a kernels for the GGUF-quantized
  * decode / prefill hot path.  Plain pointers and sizes only (device pointers unless stated);
  * no ggml, no torch, no C++ types.  Every entry point names the reference function it replaces
  * (paths relative to /root/reference/llama.cpp/).
@@ -250,7 +250,7 @@ B200_API int b200_flash_attn_any(int kv_type, const float *q, int64_t q_tok_stri
 
 /* ---- MUL_MAT, batched / prefill (replaces ggml_cuda_mul_mat_q, mmq.cu:71-143) -----------
  * dst[c][r] for any ncols; X is f32 [ncols][k].  Internally: activation quantisation as above,
- * then tiles on the tensor cores (tcgen05, TMEM accumulators) when ncols >= B200_MMQ_MIN_COLS,
+ * then tiles on the tensor cores (wgmma, register accumulators) when ncols >= B200_MMQ_MIN_COLS,
  * else column groups of 8 through the matvec kernel.  `workspace` must hold
  * b200_mul_mat_q_workspace(type,m,k,ncols) bytes. */
 B200_API int64_t b200_mul_mat_q_workspace(int type, int64_t m, int64_t k, int64_t ncols);

@@ -17,7 +17,7 @@
  * tests/test_abi.py) without the ggml tree; opaque types stand in for ggml's structs.
  *
  *   table (ggml-backend-impl.h)        implemented in llama-box_b200/plugin/ggml_b200.cpp
- *   ggml_backend_reg_i        :191-207  name "B200"; one device per sm_100 GPU; get_proc_address -> NULL
+ *   ggml_backend_reg_i        :191-207  name "B200"; one device per compute-capability 9.0 GPU; get_proc_address -> NULL
  *   ggml_backend_device_i     :137-185  type GPU; caps {async, host_buffer, events}; supports_op = the op set of
  *                                       SURVEY.md §3.3 validated node by node by b200_executor_supports();
  *                                       offload_op = false; events = cudaEvent

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for the sm_100a kernels (our code; no ggml dependency).
+// common.cuh — shared device/host helpers for the sm_90a kernels (our code; no ggml dependency).
 #pragma once
 
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// decode_mk.cu — the persistent batch-1 decode kernel (sm_100a): one launch runs a whole chain of fused phases
+// decode_mk.cu — the persistent batch-1 decode kernel (sm_90a): one launch runs a whole chain of fused phases
 // (mk.h) — [rms_norm ->] quantised matvecs with their epilogues, and rope + KV store + flash attention.
 //
 // Replaces, for a decode token, the reference's per-op launch sequence mul_mat_vec_q / quantize_q8_1 / rms_norm /

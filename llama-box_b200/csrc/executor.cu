@@ -341,8 +341,7 @@ struct Runner {
     int mk_flush_rope_only() { return rope_pend.valid ? mk_flush() : B200_OK; }
     // a decode matvec launch as a phase of the persistent kernel (Q4_K / Q6_K, one column, in-kernel activation)
     bool mk_try_mmv(const b200_mmv_launch & L) {
-        // (round 1 sent the lone 525 MB output matrix here: 5.2 vs 4.1 TB/s.  With the lean matvec instances the per-op kernel is the
-        //  faster one — 534 vs 521 tok/s — so this is opt-in now: GGML_B200_LMHEAD_MEGAKERNEL=1)
+        // (opt-in, GGML_B200_LMHEAD_MEGAKERNEL=1: with the lean matvec instances the per-op kernel is the default for the output matrix)
         static const bool big_on = getenv("GGML_B200_LMHEAD_MEGAKERNEL") != nullptr;
         const bool big = big_on && L.n_mats == 1 && !L.swiglu && (int64_t)L.mats[0].m * L.k >= ((int64_t)192 << 20) && !ex->env_no_mega && fuse;
         if (!((mega && mega_mmv) || big) || L.ncols != 1 || (L.act_source != 1 && L.act_source != 2) || L.y_out || !mk_phase_ok_k(L.k, L.act_source) || L.n_mats < 1 || L.n_mats > MK_MAX_MATS) return false;

@@ -1,4 +1,4 @@
-// fattn.cu — FLASH_ATTN_EXT over the F16 / Q8_0 KV cache, split-KV "vector" kernel (sm_100a).
+// fattn.cu — FLASH_ATTN_EXT over the F16 / Q8_0 KV cache, split-KV "vector" kernel (sm_90a).
 //
 // Replaces ggml_cuda_flash_attn_ext -> flash_attn_vec_ext_f32<D,1,K,V> + flash_attn_combine_results
 // (ggml-cuda/fattn.cu:271-338, fattn-vec-f32.cuh:10-361, fattn-common.cuh:645-701).
@@ -9,7 +9,7 @@
 //
 // Mapping: D/8 lanes per KV position (8 elements = one 16-byte load per lane for F16), so a warp
 // streams 2 (D=128) or 4 (D=64) positions per step with fully coalesced rows; up to 4 query heads of
-// one GQA group share every K/V load; KV is split over CTAs (grid.x) to fill 148 SMs, each split
+// one GQA group share every K/V load; KV is split over CTAs (grid.x) to fill the SMs (132 on an H100), each split
 // writes (m, l, acc) partials that a second kernel merges.  HBM-bound: bytes = K+V rows once per
 // head tile.
 #include "common.cuh"
@@ -531,7 +531,7 @@ int  b200_fattn_tc(const float * q, int64_t q_ts, int64_t q_hs, const void * k, 
                    float scale, float softcap, void * stream);
 
 // when the attention launch lets its dependent (the wo projection) start: 0 = at the very end, 1 = at the top (measured slower: the weight burst
-// delays the K / V loads), 2 = once every CTA has written its partials, i.e. during the split merge (default: 536 -> 549 tok/s)
+// delays the K / V loads), 2 = once every CTA has written its partials, i.e. during the split merge (default)
 static int fa_early_trigger() { static const int v = getenv("B200_FA_EARLY_TRIGGER") ? atoi(getenv("B200_FA_EARLY_TRIGGER")) : 2; return v; }
 static int fa_dispatch(const float * q, int64_t q_ts, int64_t q_hs, const void * k, int64_t k_rs, int64_t k_hs,
                                    const void * v, int64_t v_rs, int64_t v_hs, const void * mask, int64_t mask_rs, float * dst,

@@ -1,29 +1,30 @@
-// fattn_tc.cu — FLASH_ATTN_EXT for multi-token batches (prefill, large verify batches) on the tensor cores (sm_100a):
-// both contractions (S = Q K^T and O = P V) are tcgen05.mma kind::f16 with TMEM accumulators, softmax runs online in registers.
+// fattn_tc.cu — FLASH_ATTN_EXT for multi-token batches (prefill, large verify batches) on the Hopper tensor cores (sm_90a):
+// both contractions (S = Q K^T and O = P V) are wgmma m64n128k16 f16 with f32 register accumulators, softmax runs online in
+// registers.
 //
 // Replaces the multi-token path of ggml_cuda_flash_attn_ext: flash_attn_ext_f16 (ggml-cuda/fattn-mma-f16.cuh:395-1410, mma.sync
 // tiles, after a to_fp16 expansion of the WHOLE cache: fattn-common.cuh:780-833) — here K / V rows are read from the cache in
 // place, once per (query tile, head), and the decode "vec" kernel no longer re-reads the cache once per query token.
 //
 // One CTA = 128 query tokens of one head.  Per block of 128 KV positions:
-//     loader warps   K, V rows (f16, or q8_0 de-quantised to f16 d*q) -> shared memory as UMMA core matrices.  Both tiles have the
+//     loader warps   K, V rows (f16, or q8_0 de-quantised to f16 d*q) -> shared memory as core matrices.  Both tiles have the
 //                    same image [d / 8][position][8 halves]: for S = Q K^T it is the K-major B operand, for O = P V the SAME image
 //                    is an MN-major B operand (n = d, k = position), so V needs no transposition at all
-//     MMA thread     S[128 q][128 kv] = Q K^T (8 x tcgen05.mma, K = 16 over d) into TMEM
-//     softmax warps  thread = query row: s * scale + mask, online max / sum in f32 (ggml-cpu/ops.cpp:8252-8404 semantics), P =
-//                    exp(s - m) written as f16 K-major A operand; running O (f32, 128 values per thread) rescaled in registers
-//     MMA thread     O_blk[128 q][128 d] = P V (8 x tcgen05.mma, K = 16 over positions) into its own TMEM columns, added to the
-//                    running O by the softmax warps one block later
-// S and O_blk are double-buffered in TMEM (4 x 128 = all 512 columns), K / V / P tiles in shared memory.  Fully masked blocks
-// (causal future, cache padding) are skipped before anything is loaded.  Numerics: Q, K, V, P in f16 on the tensor cores
-// (the reference's CUDA path does the same); f32 softmax statistics and accumulation.  The CPU oracle keeps P in f32 and — for
-// F16 V — accumulates in fp16, so agreement is ~1e-3 relative, inside the reference harness's NMSE threshold.
+//     consumers      two warpgroups, 64 query rows each: S[64 q][128 kv] = Q K^T (8 x wgmma, K = 16 over d) into registers;
+//                    s * scale + mask, online max / sum in f32 (ggml-cpu/ops.cpp:8252-8404 semantics); P = exp(s - m) rounded
+//                    to f16 straight from the S registers into the A-operand registers of O = O * alpha + P V (8 x wgmma,
+//                    K = 16 over positions); the running O stays in the accumulator registers
+// K / V tiles are double-buffered in shared memory, so the loaders fill block i + 1 while the consumers work on block i.  Fully
+// masked blocks (causal future, cache padding) are skipped before anything is loaded.  Numerics: Q, K, V, P in f16 on the tensor
+// cores (the reference's CUDA path does the same); f32 softmax statistics and accumulation.  The CPU oracle keeps P in f32 and —
+// for F16 V — accumulates in fp16, so agreement is ~1e-3 relative, inside the reference harness's NMSE threshold.
 #include "common.cuh"
+#include "wgmma.cuh"
 
 #include <cuda_fp16.h>
 #include <math.h>
 
-#define FT_THREADS 256            // warps 0-3 softmax (255 registers available: 128 running outputs per thread), 4-6 loaders, 7 = MMA issuer + TMEM owner
+#define FT_THREADS 352            // warps 0-3 / 4-7 consumers (query rows 0-63 / 64-127), 8-10 loaders
 #define FT_PANEL 2048
 
 struct FtArgs {
@@ -37,34 +38,11 @@ struct FtArgs {
 };
 
 struct FtSmem {
-    static constexpr int Q = 0, K = 32768, V = K + 2 * 32768, P = V + 2 * 32768, BAR = P + 2 * 32768, TOTAL = BAR + 256;
+    static constexpr int Q = 0, K = 32768, V = K + 2 * 32768, BAR = V + 2 * 32768, TOTAL = BAR + 256;
 };
 
-__device__ __forceinline__ void ft_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void ft_fence_after()  { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void ft_fence_async()  { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void ft_arrive(uint64_t * bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void ft_commit(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-// K-direction / MN-direction core-matrix strides (bytes), see mmq_tc.cu
-__device__ __forceinline__ uint64_t ft_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) | (1ull << 46);
-}
-__device__ __forceinline__ void ft_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void ft_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) { return (uint32_t)__half_as_ushort(__float2half_rn(a)) | ((uint32_t)__half_as_ushort(__float2half_rn(b)) << 16); }
 
 // 8 consecutive elements of a cache row as f16 (one 16-byte K-chunk of a core matrix)
@@ -89,10 +67,8 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
     constexpr int D = 128;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t * bars = (uint64_t *)(smem + FtSmem::BAR);
-    // kv_full[2]: K,V stage loaded (128 loader threads -> 4 warp arrivals) | kv_empty[2]: MMAs reading the stage done
-    // s_full[2] / s_empty[2]: S in TMEM ready / read | p_full[2]: P tile written | o_full[2] / o_empty[2]: O_blk ready / read
-    uint64_t * kv_full = bars, * kv_empty = bars + 2, * s_full = bars + 4, * s_empty = bars + 6, * p_full = bars + 8, * o_full = bars + 10, * o_empty = bars + 12, * q_full = bars + 14;
-    uint32_t * tmem_slot = (uint32_t *)(bars + 16);
+    // kv_full[2]: K,V stage loaded (3 loader warp arrivals) | kv_empty[2]: both consumer warpgroups done with the stage
+    uint64_t * kv_full = bars, * kv_empty = bars + 2, * q_full = bars + 14;
     int * s_nblk = (int *)(bars + 17);                        // list of KV blocks that hold at least one unmasked position
     __shared__ int s_blocks[512];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -102,17 +78,10 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
     const int n_blocks_all = (a.n_kv + 127) / 128;
 
     if (tid == 0) {
-        for (int i = 0; i < 2; i++) {
-            mbar_init(&kv_full[i], 3); mbar_init(&kv_empty[i], 1); mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 4);
-            mbar_init(&p_full[i], 4); mbar_init(&o_full[i], 1); mbar_init(&o_empty[i], 4);
-        }
+        for (int i = 0; i < 2; i++) { mbar_init(&kv_full[i], 3); mbar_init(&kv_empty[i], 8); }
         mbar_init(q_full, 3);
         mbar_fence_init();
         *s_nblk = 0;
-    }
-    if (warp == 7) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     pdl_wait();
     __syncthreads();
@@ -138,18 +107,15 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
         }
         if (lane == 0 && any) s_blocks[atomicAdd(s_nblk, 1)] = b;
     }
-    ft_fence_before();
     __syncthreads();
-    ft_fence_after();
-    const uint32_t tmem = *tmem_slot;
     const int nblk = *s_nblk;
     // the list is filled in arbitrary order; every role needs the same order -> sort (tiny) by one thread
     if (tid == 0) { for (int i = 1; i < nblk; i++) { const int x = s_blocks[i]; int j = i - 1; while (j >= 0 && s_blocks[j] > x) { s_blocks[j + 1] = s_blocks[j]; j--; } s_blocks[j + 1] = x; } }
     __syncthreads();
 
-    if (warp >= 4 && warp < 7) {
+    if (warp >= 8) {
         // ===================== loaders (96 threads, rows t and t + 96): Q tile once, then K / V stages =====================
-        const int t0 = tid - 128;
+        const int t0 = tid - 256;
         for (int t = t0; t < 128; t += 96) {
             const int tok = q0 + t;
             uint8_t * Qs = smem + FtSmem::Q + t * 16;
@@ -188,155 +154,112 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
             __syncwarp();
             if (lane == 0) ft_arrive(&kv_full[st]);
         }
-    } else if (warp == 7) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            // D = f32, A = B = f16; S: both operands K-major; O: B (= V) MN-major (bit 16)
-            const uint32_t idesc_s = (1u << 4) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t idesc_o = idesc_s | (1u << 16);
-            const uint32_t qs = smem_u32(smem + FtSmem::Q);
-            mbar_wait(q_full, 0);
-            auto issue_s = [&](int i) {
-                const int st = i & 1;
-                mbar_wait(&kv_full[st], (i >> 1) & 1);
-                mbar_wait(&s_empty[st], ((i >> 1) & 1) ^ 1);
-                ft_fence_after();
-                const uint32_t ks = smem_u32(smem + FtSmem::K + st * 32768);
+    } else {
+        // ===================== consumers: warpgroup g = query rows 64 g .. 64 g + 63 =====================
+        // thread: rows ra = 64 g + 16 (warp % 4) + lane / 4 and ra + 8, columns 8 j + c0 + {0, 1} of S and of O (wgmma.cuh)
+        const int g = warp >> 2;
+        const int ra = 64 * g + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+        const uint16_t * mrow[2];
+        bool row_ok[2];
 #pragma unroll
-                for (int j = 0; j < 8; j++) ft_mma(tmem + st * 128, ft_desc(qs + j * 2 * FT_PANEL, FT_PANEL, 128), ft_desc(ks + j * 2 * FT_PANEL, FT_PANEL, 128), idesc_s, j ? 1u : 0u);
-                ft_commit(&s_full[st]);
-            };
-            if (nblk > 0) issue_s(0);
-            for (int i = 0; i < nblk; i++) {
-                const int st = i & 1;
-                if (i + 1 < nblk) issue_s(i + 1);                          // S of the next block while the softmax warps work on this one
-                mbar_wait(&p_full[st], (i >> 1) & 1);
-                mbar_wait(&o_empty[st], ((i >> 1) & 1) ^ 1);
-                ft_fence_after();
-                const uint32_t ps = smem_u32(smem + FtSmem::P + st * 32768), vs = smem_u32(smem + FtSmem::V + st * 32768);
-#pragma unroll
-                for (int j = 0; j < 8; j++)                               // K = 16 positions per MMA: P chunks 2j, 2j+1 (K-major); V position groups 2j, 2j+1 (MN-major: 128 B apart)
-                    ft_mma(tmem + 256 + st * 128, ft_desc(ps + j * 2 * FT_PANEL, FT_PANEL, 128), ft_desc(vs + j * 256, 128, FT_PANEL), idesc_o, j ? 1u : 0u);
-                ft_commit(&o_full[st]);
-                ft_commit(&kv_empty[st]);                                  // K / V stage (and P buffer) free once these MMAs have completed
-            }
+        for (int u = 0; u < 2; u++) {
+            const int tok = q0 + ra + 8 * u;
+            row_ok[u] = tok < a.n_tok;
+            mrow[u] = a.mask ? a.mask + (int64_t)(row_ok[u] ? tok : 0) * a.mask_rs : nullptr;
         }
-        __syncwarp();
-    } else if (warp < 4) {
-        // ===================== softmax + running output (thread = query row) =====================
-        const int r = warp * 32 + lane;
-        const int tok = q0 + r;
-        const bool row_ok = tok < a.n_tok;
-        const uint16_t * mrow = a.mask ? a.mask + (int64_t)(row_ok ? tok : 0) * a.mask_rs : nullptr;
-        const uint32_t lane_base = ((uint32_t)(warp * 32) << 16);
-        float O[D];
+        float O[64], S[64];
 #pragma unroll
-        for (int d = 0; d < D; d++) O[d] = 0.0f;
-        float M = -INFINITY, L = 0.0f;
+        for (int c = 0; c < 64; c++) O[c] = 0.0f;
+        float M[2] = { -INFINITY, -INFINITY }, L[2] = { 0.0f, 0.0f };           // L: this thread's share of the row sum
         const float scale = a.softcap != 0.0f ? a.scale / a.softcap : a.scale;
+        const uint32_t qs = smem_u32(smem + FtSmem::Q) + g * 1024;
+        mbar_wait(q_full, 0);
         for (int i = 0; i < nblk; i++) {
             const int st = i & 1;
             const int pb = s_blocks[i] * 128;
-            mbar_wait(&s_full[st], (i >> 1) & 1);
-            ft_fence_after();
-            // ---- pass 1: s = S * scale (+ softcap) + mask, block maximum.  S stays in TMEM; it is read again in pass 2.
-            float mloc = -INFINITY;
-#pragma unroll 1
-            for (int c0 = 0; c0 < 128; c0 += 32) {
-                uint32_t sv[32];
-                ft_ld32(tmem + lane_base + st * 128 + c0, sv);
+            mbar_wait(&kv_full[st], (i >> 1) & 1);
+            const uint32_t ks = smem_u32(smem + FtSmem::K + st * 32768), vs = smem_u32(smem + FtSmem::V + st * 32768);
+            wg_fence();
 #pragma unroll
-                for (int c = 0; c < 32; c += 8) {
-                    uint4 mk = make_uint4(0, 0, 0, 0);
-                    if (mrow) mk = *(const uint4 *)(mrow + pb + c0 + c);
-                    const uint32_t mw[4] = { mk.x, mk.y, mk.z, mk.w };
+            for (int j = 0; j < 8; j++) wg_mma_ss(S, wg_desc(qs + j * 2 * FT_PANEL, FT_PANEL, 128), wg_desc(ks + j * 2 * FT_PANEL, FT_PANEL, 128), j ? 1u : 0u);
+            wg_commit();
+            wg_wait0();
+            wg_pin(S);
+            // ---- s = S * scale (+ softcap) + mask, row maxima (a row lives in the 4 threads of a lane quad)
+            float mloc[2] = { -INFINITY, -INFINITY };
 #pragma unroll
-                    for (int e = 0; e < 8; e++) {
-                        float s = __uint_as_float(sv[c + e]) * scale;
+            for (int j = 0; j < 16; j++) {
+#pragma unroll
+                for (int u = 0; u < 2; u++) {
+                    const int col = pb + 8 * j + c0;
+                    const uint32_t mk = mrow[u] ? *(const uint32_t *)(mrow[u] + col) : 0u;
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        float s = S[4 * j + 2 * u + e] * scale;
                         if (a.softcap != 0.0f) s = a.softcap * tanhf(s);
-                        const float mv = mrow ? h2f((uint16_t)(mw[e >> 1] >> (16 * (e & 1)))) : 0.0f;
-                        s = (row_ok && pb + c0 + c + e < a.n_kv) ? s + mv : -INFINITY;
-                        mloc = fmaxf(mloc, s);
+                        const float mv = mrow[u] ? h2f((uint16_t)(mk >> (16 * e))) : 0.0f;
+                        s = (row_ok[u] && col + e < a.n_kv) ? s + mv : -INFINITY;
+                        S[4 * j + 2 * u + e] = s;
+                        mloc[u] = fmaxf(mloc[u], s);
                     }
                 }
             }
-            const float Mn = fmaxf(M, mloc);
-            const float alpha = (M == -INFINITY) ? 1.0f : expf(M - Mn);        // Mn finite here unless the whole row is masked so far (then O = L = 0 anyway)
-            // ---- pass 2: P = exp(s - Mn) as f16 into the A-operand tile, row sum
-            uint8_t * Ps = smem + FtSmem::P + st * 32768 + r * 16;
-            float lsum = 0.0f;
-#pragma unroll 1
-            for (int c0 = 0; c0 < 128; c0 += 32) {
-                uint32_t sv[32];
-                ft_ld32(tmem + lane_base + st * 128 + c0, sv);
+            float alpha[2], Mn[2];
 #pragma unroll
-                for (int c = 0; c < 32; c += 8) {
-                    uint4 mk = make_uint4(0, 0, 0, 0);
-                    if (mrow) mk = *(const uint4 *)(mrow + pb + c0 + c);
-                    const uint32_t mw[4] = { mk.x, mk.y, mk.z, mk.w };
-                    float p[8];
+            for (int u = 0; u < 2; u++) {
+                mloc[u] = fmaxf(mloc[u], __shfl_xor_sync(0xffffffffu, mloc[u], 1));
+                mloc[u] = fmaxf(mloc[u], __shfl_xor_sync(0xffffffffu, mloc[u], 2));
+                Mn[u] = fmaxf(M[u], mloc[u]);
+                alpha[u] = (M[u] == -INFINITY) ? 1.0f : expf(M[u] - Mn[u]);     // Mn finite here unless the whole row is masked so far (then O = L = 0 anyway)
+            }
+            // ---- P = exp(s - Mn) rounded to f16: the A operand of P V, straight from the S registers
+            uint32_t P[8][4];
+            float lsum[2] = { 0.0f, 0.0f };
 #pragma unroll
-                    for (int e = 0; e < 8; e++) {
-                        float s = __uint_as_float(sv[c + e]) * scale;
-                        if (a.softcap != 0.0f) s = a.softcap * tanhf(s);
-                        const float mv = mrow ? h2f((uint16_t)(mw[e >> 1] >> (16 * (e & 1)))) : 0.0f;
-                        s = (row_ok && pb + c0 + c + e < a.n_kv) ? s + mv : -INFINITY;
-                        p[e] = (Mn == -INFINITY) ? 0.0f : expf(s - Mn);
+            for (int j = 0; j < 16; j++) {
+#pragma unroll
+                for (int u = 0; u < 2; u++) {
+                    float p[2];
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        p[e] = (Mn[u] == -INFINITY) ? 0.0f : expf(S[4 * j + 2 * u + e] - Mn[u]);
                         // the tensor core sees f16(p): sum the SAME rounded values so that O / L is a proper weighted mean
                         p[e] = __half2float(__float2half_rn(p[e]));
-                        lsum += p[e];
+                        lsum[u] += p[e];
                     }
-                    uint4 o; o.x = pack_h2(p[0], p[1]); o.y = pack_h2(p[2], p[3]); o.z = pack_h2(p[4], p[5]); o.w = pack_h2(p[6], p[7]);
-                    *(uint4 *)(Ps + ((c0 + c) >> 3) * FT_PANEL) = o;
+                    P[j >> 1][(j & 1) * 2 + u] = pack_h2(p[0], p[1]);
                 }
             }
-            ft_fence_before();
-            ft_fence_async();
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+#pragma unroll
+                for (int u = 0; u < 2; u++) { O[4 * j + 2 * u] *= alpha[u]; O[4 * j + 2 * u + 1] *= alpha[u]; }
+            }
+#pragma unroll
+            for (int u = 0; u < 2; u++) { L[u] = L[u] * alpha[u] + lsum[u]; M[u] = Mn[u]; }
+            wg_fence();
+#pragma unroll
+            for (int kk = 0; kk < 8; kk++)                                      // K = 16 positions per MMA; V position groups 2kk, 2kk+1 (MN-major: 128 B apart)
+                wg_mma_rs_bmn(O, P[kk], wg_desc(vs + kk * 256, 128, FT_PANEL), 1u);
+            wg_commit();
+            wg_wait0();
+            wg_pin(O);
             __syncwarp();
-            if (lane == 0) { ft_arrive(&s_empty[st]); ft_arrive(&p_full[st]); }
-            // ---- fold in the PREVIOUS block's P V (it is relative to the previous maximum), then move everything to the new maximum
-            if (i > 0) {
-                const int sp = (i - 1) & 1;
-                mbar_wait(&o_full[sp], ((i - 1) >> 1) & 1);
-                ft_fence_after();
-#pragma unroll
-                for (int c0 = 0; c0 < D; c0 += 32) {
-                    uint32_t ov[32];
-                    ft_ld32(tmem + lane_base + 256 + sp * 128 + c0, ov);
-#pragma unroll
-                    for (int c = 0; c < 32; c++) O[c0 + c] += __uint_as_float(ov[c]);
-                }
-                ft_fence_before();
-                __syncwarp();
-                if (lane == 0) ft_arrive(&o_empty[sp]);
-            }
-#pragma unroll
-            for (int d = 0; d < D; d++) O[d] *= alpha;
-            L = L * alpha + lsum; M = Mn;
+            if (lane == 0) ft_arrive(&kv_empty[st]);                            // K / V stage free
         }
-        if (nblk > 0) {
-            const int sp = (nblk - 1) & 1;
-            mbar_wait(&o_full[sp], ((nblk - 1) >> 1) & 1);
-            ft_fence_after();
 #pragma unroll
-            for (int c0 = 0; c0 < D; c0 += 32) {
-                uint32_t ov[32];
-                ft_ld32(tmem + lane_base + 256 + sp * 128 + c0, ov);
+        for (int u = 0; u < 2; u++) {
+            float l = L[u];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            if (!row_ok[u]) continue;
+            const float inv = l > 0.0f ? 1.0f / l : 0.0f;                        // ops.cpp:8390-8392 (V /= S)
+            float * out = a.dst + ((int64_t)(q0 + ra + 8 * u) * a.n_head + h) * D;
 #pragma unroll
-                for (int c = 0; c < 32; c++) O[c0 + c] += __uint_as_float(ov[c]);
-            }
-        }
-        if (row_ok) {
-            const float inv = L > 0.0f ? 1.0f / L : 0.0f;                      // ops.cpp:8390-8392 (V /= S)
-            float * out = a.dst + ((int64_t)tok * a.n_head + h) * D;
-#pragma unroll
-            for (int d = 0; d < D; d += 4) *(float4 *)(out + d) = make_float4(O[d] * inv, O[d + 1] * inv, O[d + 2] * inv, O[d + 3] * inv);
+            for (int j = 0; j < 16; j++) *(float2 *)(out + 8 * j + c0) = make_float2(O[4 * j + 2 * u] * inv, O[4 * j + 2 * u + 1] * inv);
         }
     }
     pdl_trigger();
-    ft_fence_before();
-    __syncthreads();
-    if (warp == 7) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(512u) : "memory");
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------

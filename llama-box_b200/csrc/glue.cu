@@ -1,4 +1,4 @@
-// glue.cu — the small elementwise ops that keep a whole transformer layer on the device (sm_100a).
+// glue.cu — the small elementwise ops that keep a whole transformer layer on the device (sm_90a).
 // Replaces k_bin_bcast (ggml-cuda/binbcast.cu:26-93), unary_gated_op_kernel (unary.cu:209-230),
 // k_get_rows_float (getrows.cu:5-67), cpy_flt f32->f16 (cpy.cu:11-64) and argmax (argmax.cu).
 // All HBM/launch-bound: 16-byte vector accesses, grid sized to the data, f32 math in the oracle's

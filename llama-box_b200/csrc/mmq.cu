@@ -1,6 +1,6 @@
 // mmq.cu — batched MUL_MAT on quantised weights (prefill / ubatches of more than 8 tokens), host dispatch.
 // Replaces ggml_cuda_mul_mat_q (ggml-cuda/mmq.cu:71-143).
-//   * K-quants (Q4_K / Q5_K / Q6_K): the tcgen05 tile kernel of mmq_tc.cu (tensor cores, TMEM accumulators, TMA staging),
+//   * K-quants (Q4_K / Q5_K / Q6_K): the wgmma tile kernel of mmq_tc.cu (tensor cores, register accumulators, TMA staging),
 //     integer-exact against the CPU oracle;
 //   * Q4_0 / Q8_0 (per-32 f16 block scales): activations quantised like the CPU oracle (quantize.cu) and columns streamed
 //     through the matvec kernel in groups of 8 (weights re-read from L2 / HBM per group).

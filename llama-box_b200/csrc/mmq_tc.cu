@@ -1,5 +1,5 @@
-// mmq_tc.cu — batched MUL_MAT on K-quant weights (prefill / large ubatches) on the 5th-generation tensor cores (sm_100a):
-// tcgen05.mma with TMEM accumulators, TMA (cp.async.bulk) staging, warp-specialised, persistent.
+// mmq_tc.cu — batched MUL_MAT on K-quant weights (prefill / large ubatches) on the Hopper tensor cores (sm_90a):
+// wgmma with register accumulators, TMA (cp.async.bulk) staging, warp-specialised, persistent.
 //
 // Replaces ggml_cuda_mul_mat_q / mul_mat_q<type,mmq_x> (ggml-cuda/mmq.cu:71-143, mmq.cuh:3047-3370: int8 mma.sync tiles
 // with per-32 f32 scale FMAs in the inner loop, stream-K fixup :3373-3522) and quantize_mmq_q8_1 (quantize.cu:50-146).
@@ -12,29 +12,28 @@
 //
 //   * A operand (weights): a transform warpgroup unpacks the packed quants from shared memory into f16 INTEGERS with the
 //     6-bit sub-block scale folded in, a[r][k] = sc_j * q  (<= 63*15 = 945 for Q4_K, <= 63*31 = 1953 for Q5_K: exact in f16),
-//     written as UMMA K-major core matrices.  Q6_K's sc * (q - 32) reaches +-4096, which f16 holds only when even: the
+//     written as K-major core matrices.  Q6_K's sc * (q - 32) reaches +-4096, which f16 holds only when even: the
 //     product is split as (sc & ~1) * (q - 32)  [even, exact]  +  (sc & 1) * (q - 32)  [|.| <= 32], two K-passes into ONE
 //     accumulator.
 //   * B operand (activations): q8 values as f16 integers (|q8| <= 127), pre-tiled in HBM in the exact shared-memory image so
 //     that one bulk copy brings a [128 tokens x 64 k] panel.
-//   * tcgen05.mma kind::f16, M = 128, N <= 128, K = 16 per instruction, f32 accumulate in TMEM: every product and every
-//     partial sum is an integer below 2^24, so the accumulation is EXACT and isum equals the oracle's int32 bit for bit.
-//     imin is one more K = 16 MMA per super-block (A = m_j as f16, B = the q8_K bsums as f16) into its own TMEM columns.
-//   * epilogue warps drain TMEM once per super-block (tcgen05.ld), apply d_w * d_x and dmin_w * d_x in f32 — the only
-//     floating-point rounding on the path, the same two roundings per super-block the oracle performs — and keep the f32
-//     running sums in registers.  TMEM is double-buffered (2 x (isum 128 cols + imin 128 cols) = all 512 columns), so the
-//     drain of super-block s overlaps the MMAs of s + 1.
+//   * wgmma m64n128k16 f16, f32 accumulate in registers: every product and every partial sum is an integer below 2^24, so the
+//     accumulation is EXACT and isum equals the oracle's int32 bit for bit.  imin is one more K = 16 MMA per super-block
+//     (A = m_j as f16, B = the q8_K bsums as f16) into the same registers once isum has been folded in.
+//   * the consumer warpgroups fold each super-block into f32 running sums in registers: acc += (d_w * d_x) * isum, then
+//     acc -= (dmin_w * d_x) * imin — the floating-point roundings of the oracle's two products, with the difference applied
+//     to the running sum in two steps (an isum and an imin accumulator do not both fit in the register file next to acc).
 //
-// Warp roles (448 threads, one persistent CTA per SM):
-//     warps 0-3 / 4-7  epilogue, columns 0-63 / 64-127 (warp % 4 = TMEM lane quadrant)
+// Warp roles (384 threads, one persistent CTA per SM):
+//     warps 0-3 / 4-7  consumers: tile rows 0-63 / 64-127, all 128 columns (issue the MMAs, fold, store)
 //     warps 8-11       transform: thread t owns weight row t of the tile; packed blocks come straight from global memory into
-//                      registers, one super-block ahead
-//     warp 12          TMA producer: the activation panels of each stage (cp.async.bulk, mbarrier complete_tx)
-//     warp 13          TMEM allocation + the single MMA-issuing thread
-// Shared memory (per CTA): 2 A stages x 32 KB (128 rows x 128 k f16) + 2 B stages x 32 KB + raw weight blocks x 2 + the
-// imin operands + scale rings, ~200 KB.  Data movement: weights are read from HBM once per 128-token tile (L2 serves the
-// other token tiles of the same rows, which run on neighbouring CTAs), activations stream from L2.
+//                      registers, one super-block ahead; thread 0 also issues the activation panels of each stage
+//                      (cp.async.bulk, mbarrier complete_tx) as soon as the stage is free
+// Shared memory (per CTA, ~150 KB): 2 A stages x 32 KB (128 rows x 128 k f16) + 2 B stages x 32 KB + the imin operands + scale rings.
+// Data movement: weights are read from HBM once per 128-token tile (L2 serves the other token tiles of the same rows, which
+// run on neighbouring CTAs), activations stream from L2.
 #include "common.cuh"
+#include "wgmma.cuh"
 
 #include <cuda_fp16.h>
 #include <cstdio>
@@ -42,7 +41,7 @@
 
 #define TC_TM 128
 #define TC_TN 128
-#define TC_THREADS 448
+#define TC_THREADS 384
 #define TC_STAGE_A 32768
 #define TC_STAGE_B 32768
 #define TC_PANEL 2048             // one K-chunk (8 f16 = 16 bytes) of 128 rows
@@ -116,34 +115,10 @@ __global__ void __launch_bounds__(256) quantize_mmq_kernel(const float * __restr
     pdl_trigger();
 }
 
-// ---- tcgen05 / TMEM primitives (inline PTX; SASS: UTCHMMA, LDTM, UTCBAR, ...) -------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after()  { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint64_t * bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_commit(uint64_t * bar) {          // arrives on `bar` when every MMA issued so far by this thread has completed
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-// shared-memory matrix descriptor, K-major, no swizzle ("interleaved" core matrices of 8 rows x 16 bytes):
-//   element (row r, 16-byte K-chunk c) lives at  start + c * LBO + (r / 8) * SBO + (r % 8) * 16
-// (cute::UMMA::SmemDescriptor, canonical layout ((8,n),2):((1,SBO),LBO) in 16-byte units; bits 46-47 = 1 on sm_100)
-__device__ __forceinline__ uint64_t tc_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) | (1ull << 46);
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 struct TcArgs {
     const uint8_t * W;          // weights, `type` rows (Q6_K: repacked rows, see repack.cu)
@@ -161,22 +136,18 @@ __device__ __forceinline__ void mbar_wait_p(uint64_t * bar, uint32_t parity, uns
     else mbar_wait(bar, parity);
 }
 
-// ---- per-type geometry of the raw (packed) weight blocks staged in shared memory ------------------------------------
+// ---- per-type pipeline geometry: K-stages per super-block, whether the mins MMA runs, activation bytes per stage -------
+// (the transform threads read each row's packed blocks straight from global memory, so no weight bytes live in shared memory;
+// Q6_K rows are repacked [ql 128B x nb][qh 64B x nb][scales 16B x nb][d f16 x nb], see repack.cu)
 template <int T> struct TcType;
-// RAW_SLOTS: depth of the packed-weight ring.  The raw producer warp runs ahead of everything else (its only dependency is
-// the transform having consumed a slot), so that HBM latency of the weight stream is hidden behind RAW_SLOTS - 1 super-blocks
-template <> struct TcType<B200_TYPE_Q4_K> { static constexpr int STAGES = 2, RAW = 128 * 144, HAS_MIN = 1, B_BYTES = 32768, RAW_SLOTS = 4; };
-template <> struct TcType<B200_TYPE_Q5_K> { static constexpr int STAGES = 2, RAW = 128 * 176, HAS_MIN = 1, B_BYTES = 32768, RAW_SLOTS = 3; };
-// Q6_K rows are repacked [ql 128B x nb][qh 64B x nb][scales 16B x nb][d f16 x nb]; staged with padded row strides
-// (144 / 80 / 16 bytes) so that thread-per-row 16-byte reads are bank-conflict free; d is fetched 8 super-blocks at a time
-template <> struct TcType<B200_TYPE_Q6_K> { static constexpr int STAGES = 4, RAW = 128 * (144 + 80 + 16), HAS_MIN = 0, B_BYTES = 16384, RAW_SLOTS = 2; };
+template <> struct TcType<B200_TYPE_Q4_K> { static constexpr int STAGES = 2, HAS_MIN = 1, B_BYTES = 32768; };
+template <> struct TcType<B200_TYPE_Q5_K> { static constexpr int STAGES = 2, HAS_MIN = 1, B_BYTES = 32768; };
+template <> struct TcType<B200_TYPE_Q6_K> { static constexpr int STAGES = 4, HAS_MIN = 0, B_BYTES = 16384; };
 
 // shared memory map
 struct TcSmem {
-    static constexpr int A = 0, B = A + 2 * TC_STAGE_A, AM = B + 2 * TC_STAGE_B, BM = AM + 2 * 4096, RAWO = BM + 2 * 4096;
-    static constexpr int RAW_BYTES = 73728;                  // ring of packed weight blocks: 4 x 18 KB (Q4_K), 3 x 22 KB (Q5_K), 2 x 30 KB (Q6_K)
-    static constexpr int DC = RAWO + RAW_BYTES;              // Q6_K d cache: 2 x 128 rows x 16 B
-    static constexpr int RS = DC + 2 * 2048;                 // row scales ring: 4 x 128 x float2
+    static constexpr int A = 0, B = A + 2 * TC_STAGE_A, AM = B + 2 * TC_STAGE_B, BM = AM + 2 * 4096;
+    static constexpr int RS = BM + 2 * 4096;                 // row scales ring: 4 x 128 x float2
     static constexpr int D8 = RS + 4 * 1024;                 // d_x ring: 4 x 128 f32
     static constexpr int BAR = D8 + 4 * 512;                 // mbarriers
     static constexpr int TOTAL = BAR + 256;
@@ -201,104 +172,45 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
     using TT = TcType<T>;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t * bars = (uint64_t *)(smem + TcSmem::BAR);
-    uint64_t * raw_full = bars, * raw_empty = bars + 4, * b_full = bars + 8, * a_full = bars + 10, * ab_empty = bars + 12, * acc_full = bars + 14, * acc_empty = bars + 16;
-    uint32_t * tmem_slot = (uint32_t *)(bars + 18);
-    constexpr int RSL = TT::RAW_SLOTS;
+    uint64_t * b_full = bars + 8, * a_full = bars + 10, * ab_empty = bars + 12;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
     if (tid == 0) {
-        for (int i = 0; i < 4; i++) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], 4); }
-        for (int i = 0; i < 2; i++) {
-            mbar_init(&b_full[i], 1); mbar_init(&a_full[i], 4);
-            mbar_init(&ab_empty[i], 1); mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 8);
-        }
+        for (int i = 0; i < 2; i++) { mbar_init(&b_full[i], 1); mbar_init(&a_full[i], 4); mbar_init(&ab_empty[i], 8); }
         mbar_fence_init();
     }
-    if (warp == 13) {                                              // TMEM: all 512 columns (one CTA per SM)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_wait();
 
     const int nsb = args.nsb;
     const int64_t NT = args.g.nt;
-    unsigned long long w0 = 0, w1 = 0, w2 = 0;                       // profile: cycles in this role's three kinds of waits
+    unsigned long long w0 = 0, w1 = 0, w2 = 0;                       // profile: cycles in this role's kinds of waits
     const bool prof = args.prof != nullptr && blockIdx.x == 0;
-    unsigned long long * pw0 = prof ? &w0 : nullptr, * pw1 = prof ? &w1 : nullptr, * pw2 = prof ? &w2 : nullptr;
+    unsigned long long * pw0 = prof ? &w0 : nullptr, * pw1 = prof ? &w1 : nullptr;
     const long long t_start = clock64();
 
-    if (warp == 12) {
-        // ===================== TMA producer: activation panels, one per stage (+ the bsum panel and d_x with the first) =====================
-        uint32_t it = 0, sbc = 0;
-        for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
-            const int64_t nt = tile % NT;
-            for (int sb = 0; sb < nsb; sb++, sbc++) {
-                const int rs = sbc & 1;
-                for (int s = 0; s < TT::STAGES; s++, it++) {
-                    const int st = it & 1;
-                    mbar_wait_p(&ab_empty[st], ((it >> 1) & 1) ^ 1, pw0);
-                    if (lane == 0) {
-                        const uint32_t extra = s == 0 ? (512u + (TT::HAS_MIN ? 4096u : 0u)) : 0u;
-                        mbar_expect_tx(&b_full[st], (uint32_t)TT::B_BYTES + extra);
-                        const int64_t kq0 = (int64_t)sb * 4 + (TT::STAGES == 2 ? s * 2 : s);
-                        const uint8_t * src = args.ws + args.g.off_bq + (nt * args.g.kq + kq0) * 16384;
-                        uint8_t * dstb = smem + TcSmem::B + st * TC_STAGE_B;
-                        for (int o = 0; o < TT::B_BYTES; o += 8192) bulk_g2s(dstb + o, src + o, 8192, &b_full[st]);
-                        if (s == 0) {
-                            if (TT::HAS_MIN) bulk_g2s(smem + TcSmem::BM + rs * 4096, args.ws + args.g.off_bm + (nt * nsb + sb) * 4096, 4096, &b_full[st]);
-                            bulk_g2s(smem + TcSmem::D8 + (sbc & 3) * 512, args.ws + args.g.off_d8 + (nt * nsb + sb) * 512, 512, &b_full[st]);
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
+    // activation panels of one stage (+ the bsum panel and d_x with the first stage of a super-block), issued by one thread of
+    // the transform warpgroup once the stage is free (cp.async.bulk, mbarrier complete_tx)
+    auto load_b = [&](int64_t nt, int sb, uint32_t sbc, int s, int st) {
+        const uint32_t extra = s == 0 ? (512u + (TT::HAS_MIN ? 4096u : 0u)) : 0u;
+        mbar_expect_tx(&b_full[st], (uint32_t)TT::B_BYTES + extra);
+        const int64_t kq0 = (int64_t)sb * 4 + (TT::STAGES == 2 ? s * 2 : s);
+        const uint8_t * src = args.ws + args.g.off_bq + (nt * args.g.kq + kq0) * 16384;
+        uint8_t * dstb = smem + TcSmem::B + st * TC_STAGE_B;
+        for (int o = 0; o < TT::B_BYTES; o += 8192) bulk_g2s(dstb + o, src + o, 8192, &b_full[st]);
+        if (s == 0) {
+            if (TT::HAS_MIN) bulk_g2s(smem + TcSmem::BM + (sbc & 1) * 4096, args.ws + args.g.off_bm + (nt * nsb + sb) * 4096, 4096, &b_full[st]);
+            bulk_g2s(smem + TcSmem::D8 + (sbc & 3) * 512, args.ws + args.g.off_d8 + (nt * nsb + sb) * 512, 512, &b_full[st]);
         }
-    } else if (warp == 13) {
-        // ===================== MMA issuer (one thread) =====================
-        if (lane == 0) {
-            uint32_t it = 0, sbc = 0;
-            for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
-                const int64_t nt = tile % NT;
-                const int64_t nval = args.ncols - nt * TC_TN < TC_TN ? args.ncols - nt * TC_TN : TC_TN;
-                const uint32_t n_eff = (uint32_t)((nval + 15) & ~15);
-                // instruction descriptor (cute::UMMA::InstrDescriptor): D = f32, A = B = f16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-                const uint32_t idesc = (1u << 4) | ((n_eff >> 3) << 17) | ((uint32_t)(TC_TM >> 4) << 24);
-                for (int sb = 0; sb < nsb; sb++, sbc++) {
-                    const int rs = sbc & 1;
-                    mbar_wait_p(&acc_empty[rs], ((sbc >> 1) & 1) ^ 1, pw0);       // epilogue has drained this TMEM buffer
-                    tc_fence_after();
-                    const uint32_t d_main = tmem + rs * 128, d_min = tmem + 256 + rs * 128;
-                    for (int s = 0; s < TT::STAGES; s++, it++) {
-                        const int st = it & 1; const uint32_t ph = (it >> 1) & 1;
-                        mbar_wait_p(&b_full[st], ph, pw1);
-                        mbar_wait_p(&a_full[st], ph, pw2);
-                        tc_fence_after();
-                        const uint32_t a0 = smem_u32(smem + TcSmem::A + st * TC_STAGE_A), b0 = smem_u32(smem + TcSmem::B + st * TC_STAGE_B);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            const uint32_t bj = TT::STAGES == 2 ? j : (j & 3);    // Q6_K: the even and the odd-scale pass read the same 64-k panel
-                            tc_mma_f16(d_main, tc_desc(a0 + j * 2 * TC_PANEL, args.lbo, args.sbo), tc_desc(b0 + bj * 2 * TC_PANEL, args.lbo, args.sbo), idesc, (s | j) ? 1u : 0u);
-                        }
-                        if (TT::HAS_MIN && s == TT::STAGES - 1)
-                            tc_mma_f16(d_min, tc_desc(smem_u32(smem + TcSmem::AM + rs * 4096), args.lbo, args.sbo), tc_desc(smem_u32(smem + TcSmem::BM + rs * 4096), args.lbo, args.sbo), idesc, 0u);
-                        tc_commit(&ab_empty[st]);                          // stage buffers reusable once these MMAs have completed
-                    }
-                    tc_commit(&acc_full[rs]);                              // accumulators of this super-block complete
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp >= 8 && warp < 12) {
+    };
+
+    if (warp >= 8) {
         // ===================== transform: packed quants -> f16 sc*q core matrices =====================
         // Thread t owns weight row t of the tile and reads its packed block of the NEXT super-block straight from global memory
         // into registers (9-14 16-byte loads, issued one super-block ahead, so HBM / L2 latency hides behind the conversion of
         // the current one).  (A first version staged the blocks through shared memory with one cp.async.bulk per row: a
         // warp-wide bulk copy is issued lane by lane through uniform registers, ~65 cycles each — 128 rows cost 8 K cycles per
-        // super-block and starved everything else; profiles/README.md.)
+        // super-block and starved everything else.)
         constexpr int NW = T == B200_TYPE_Q4_K ? 9 : (T == B200_TYPE_Q5_K ? 11 : 13);
         const int t = tid - 8 * 32;                                      // weight row of the tile
         const int64_t nb = args.k / 256;
@@ -346,6 +258,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                     for (int s = 0; s < 2; s++, it++) {                   // half super-block = 128 k = one stage
                         const int st = it & 1;
                         mbar_wait_p(&ab_empty[st], ((it >> 1) & 1) ^ 1, pw1);
+                        if (t == 0) load_b(tile % NT, sb, sbc, s, st);
                         uint8_t * As = smem + TcSmem::A + st * TC_STAGE_A + t * 16;
 #pragma unroll
                         for (int gg = 0; gg < 2; gg++) {
@@ -397,6 +310,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                     for (int s = 0; s < 4; s++, it++) {                   // quarter super-block = 64 k: chunks 0-7 = even-scale part, 8-15 = odd-scale part
                         const int st = it & 1;
                         mbar_wait_p(&ab_empty[st], ((it >> 1) & 1) ^ 1, pw1);
+                        if (t == 0) load_b(tile % NT, sb, sbc, s, st);
                         uint8_t * As = smem + TcSmem::A + st * TC_STAGE_A + t * 16;
                         const int hh = s >> 1, u2 = s & 1;
                         const uint4 qha = cur[8 + hh * 2], qhb = cur[8 + hh * 2 + 1];
@@ -436,50 +350,78 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
             }
         }
     } else {
-        // ===================== epilogue: TMEM -> f32 running sums in registers -> dst =====================
-        const int quad = warp & 3, ch = warp >> 2;
-        const int r = quad * 32 + lane;                                   // tile row = TMEM lane
-        uint32_t sbc = 0;
+        // ===================== consumers: MMAs of rows 64 g .. 64 g + 63, fold into f32 running sums, store =====================
+        const int g = warp >> 2;
+        const int ra = 64 * g + 16 * (warp & 3) + (lane >> 2);          // tile rows ra, ra + 8 (wgmma accumulator layout, wgmma.cuh)
+        const int c0 = 2 * (lane & 3);                                  // tile columns 8 j + c0 + {0, 1}
+        const uint64_t dmin_a = wg_desc(smem_u32(smem + TcSmem::AM + g * 1024), args.lbo, args.sbo);
+        uint32_t it = 0, sbc = 0;
         for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
             const int64_t mt = tile / NT, nt = tile % NT;
-            const int64_t nval = args.ncols - nt * TC_TN < TC_TN ? args.ncols - nt * TC_TN : TC_TN;
-            const int n_eff = (int)((nval + 15) & ~15);
-            float acc[64];
+            float acc[64], frag[64];
 #pragma unroll
             for (int c = 0; c < 64; c++) acc[c] = 0.0f;
             for (int sb = 0; sb < nsb; sb++, sbc++) {
                 const int rs = sbc & 1;
-                mbar_wait_p(&acc_full[rs], (sbc >> 1) & 1, pw0);
-                tc_fence_after();
-                const float2 dd = ((const float2 *)(smem + TcSmem::RS + (sbc & 3) * 1024))[r];
-                const float * d8 = (const float *)(smem + TcSmem::D8 + (sbc & 3) * 512) + ch * 64;
-                const uint32_t tbase = tmem + ((uint32_t)(quad * 32) << 16) + rs * 128 + ch * 64;
+                for (int s = 0; s < TT::STAGES; s++, it++) {
+                    const int st = it & 1; const uint32_t ph = (it >> 1) & 1;
+                    mbar_wait_p(&b_full[st], ph, pw0);
+                    mbar_wait_p(&a_full[st], ph, pw1);
+                    const uint32_t a0 = smem_u32(smem + TcSmem::A + st * TC_STAGE_A) + g * 1024, b0 = smem_u32(smem + TcSmem::B + st * TC_STAGE_B);
+                    wg_fence();
 #pragma unroll
-                for (int c0 = 0; c0 < 64; c0 += 16) {
-                    if (ch * 64 + c0 < n_eff) {                            // warp-uniform
-                        uint32_t vm[16], vn[16];
-                        tc_ld16(tbase + c0, vm);
-                        if (TT::HAS_MIN) tc_ld16(tbase + 256 + c0, vn);
-                        tc_ld_wait();
+                    for (int j = 0; j < 8; j++) {
+                        const uint32_t bj = TT::STAGES == 2 ? j : (j & 3);        // Q6_K: the even and the odd-scale pass read the same 64-k panel
+                        wg_mma_ss(frag, wg_desc(a0 + j * 2 * TC_PANEL, args.lbo, args.sbo), wg_desc(b0 + bj * 2 * TC_PANEL, args.lbo, args.sbo), (s | j) ? 1u : 0u);
+                    }
+                    wg_commit();
+                    wg_wait0();
+                    wg_pin(frag);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&ab_empty[st]);                  // stage buffers reusable
+                }
+                // the scale rings (4 deep) and the imin operands (2 deep) of this super-block stay valid until this warpgroup has
+                // released the stages of super-block sb + 1, which it does only after this fold
+                const float2 * rsc = (const float2 *)(smem + TcSmem::RS + (sbc & 3) * 1024);
+                const float2 da = rsc[ra], db = rsc[ra + 8];
+                const float * d8 = (const float *)(smem + TcSmem::D8 + (sbc & 3) * 512);
 #pragma unroll
-                        for (int c = 0; c < 16; c++) {
-                            const float dx = d8[c0 + c];
-                            float u = __fmul_rn(__fmul_rn(dd.x, dx), __uint_as_float(vm[c]));               // d * isum       (ggml-cpu/quants.c:615-620)
-                            if (TT::HAS_MIN) u = __fsub_rn(u, __fmul_rn(__fmul_rn(dd.y, dx), __uint_as_float(vn[c])));   // - dmin * imin
-                            acc[c0 + c] = __fadd_rn(acc[c0 + c], u);
+                for (int j = 0; j < 16; j++) {
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const float dx = d8[8 * j + c0 + e];
+                        acc[4 * j + e]     = __fadd_rn(acc[4 * j + e],     __fmul_rn(__fmul_rn(da.x, dx), frag[4 * j + e]));       // d * isum (ggml-cpu/quants.c:615-620)
+                        acc[4 * j + 2 + e] = __fadd_rn(acc[4 * j + 2 + e], __fmul_rn(__fmul_rn(db.x, dx), frag[4 * j + 2 + e]));
+                    }
+                }
+                if (TT::HAS_MIN) {
+                    wg_fence();
+                    wg_mma_ss(frag, dmin_a + ((uint64_t)(rs * 4096) >> 4), wg_desc(smem_u32(smem + TcSmem::BM + rs * 4096), args.lbo, args.sbo), 0u);
+                    wg_commit();
+                    wg_wait0();
+                    wg_pin(frag);
+#pragma unroll
+                    for (int j = 0; j < 16; j++) {
+#pragma unroll
+                        for (int e = 0; e < 2; e++) {
+                            const float dx = d8[8 * j + c0 + e];
+                            acc[4 * j + e]     = __fsub_rn(acc[4 * j + e],     __fmul_rn(__fmul_rn(da.y, dx), frag[4 * j + e]));   // - dmin * imin
+                            acc[4 * j + 2 + e] = __fsub_rn(acc[4 * j + 2 + e], __fmul_rn(__fmul_rn(db.y, dx), frag[4 * j + 2 + e]));
                         }
                     }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[rs]);
             }
-            const int64_t row = mt * TC_TM + r;
-            if (row < args.m) {
 #pragma unroll
-                for (int c = 0; c < 64; c++) {
-                    const int64_t n = nt * TC_TN + ch * 64 + c;
-                    if (n < args.ncols) args.dst[n * args.ldd + row] = acc[c];
+            for (int h = 0; h < 2; h++) {
+                const int64_t row = mt * TC_TM + ra + 8 * h;
+                if (row >= args.m) continue;
+#pragma unroll
+                for (int j = 0; j < 16; j++) {
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int64_t n = nt * TC_TN + 8 * j + c0 + e;
+                        if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
+                    }
                 }
             }
         }
@@ -489,11 +431,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
         unsigned long long * o = args.prof + warp * 4;
         o[0] = (unsigned long long)(clock64() - t_start); o[1] = w0; o[2] = w1; o[3] = w2;
     }
-    // ---- teardown
     pdl_trigger();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 13) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(512u) : "memory");
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
@@ -541,11 +479,11 @@ int b200_mmq_tc(int type, const void * W, const float * X, int64_t x_col_stride,
     if (want_prof && rc == B200_OK) {
         unsigned long long h[16 * 4];
         cudaStreamSynchronize(st); cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
-        const char * role[14] = { "epi", "epi", "epi", "epi", "epi", "epi", "epi", "epi", "xform", "xform", "xform", "xform", "b-tma", "mma" };
+        const char * role[12] = { "mma", "mma", "mma", "mma", "mma", "mma", "mma", "mma", "xform", "xform", "xform", "xform" };
         fprintf(stderr, "mmq_tc prof (CTA 0, cycles): type %d m %lld k %lld n %lld tiles %d\n", type, (long long)m, (long long)k, (long long)ncols, a.n_tiles);
-        for (int w = 0; w < 14; w += (w < 8 ? 4 : (w < 12 ? 2 : 1)))
+        for (int w = 0; w < 12; w += (w < 8 ? 4 : 2))
             fprintf(stderr, "  warp %2d %-8s total %9llu  wait0 %9llu  wait1 %9llu  wait2 %9llu\n", w, role[w], h[w * 4], h[w * 4 + 1], h[w * 4 + 2], h[w * 4 + 3]);
-        fprintf(stderr, "  (epi: wait0 = acc_full | xform: wait1 = ab_empty | mma: wait0 = acc_empty, wait1 = b_full, wait2 = a_full | b-tma: wait0 = ab_empty)\n");
+        fprintf(stderr, "  (mma: wait0 = b_full, wait1 = a_full | xform: wait1 = ab_empty)\n");
     }
     return rc;
 }

@@ -1,4 +1,4 @@
-// mmvq.cu — decode matvec on GGUF-quantised weights (sm_100a), ncols <= 8.
+// mmvq.cu — decode matvec on GGUF-quantised weights (sm_90a), ncols <= 8.
 //
 // Replaces ggml_cuda_mul_mat_vec_q / mul_mat_vec_q<type,ncols_dst> (ggml-cuda/mmvq.cu:139-226,
 // 500-570) and vec_dot_q*_q8_1 (vecdotq.cuh:579-839).  Design (HBM-bound; bytes = m * row_bytes):
@@ -24,7 +24,7 @@
 #define MMV_WARPS 16
 #endif
 #ifndef MMV_CTAS_PER_SM
-#define MMV_CTAS_PER_SM 1      // 8 warps x 2 CTAs of 108 KB (so that the next launch primes its ring next to this one) was measured: 300 tok/s instead of 400
+#define MMV_CTAS_PER_SM 1      // one CTA of 16 warps per SM: the whole warp count keeps the bulk copies of the ring in flight
 #endif
 #define MMV_MAX_MATS 4
 #define MMV_MAX_STAGES 8
@@ -253,7 +253,7 @@ template <> struct WChunk<B200_TYPE_Q6_K> {
 
 // ---- fast paths for 2048-element segments (segc == 64: 8 super-blocks per row segment) -------------
 // The generic WChunk code above spends ~100 instructions per 32 weights (6-bit scale unpack and nibble
-// shifts per chunk), which makes the matvec ISSUE-bound long before HBM is saturated (ncu: 2 TB/s).
+// shifts per chunk), which makes the matvec ISSUE-bound long before HBM is saturated.
 // Here one lane owns 64 elements of ONE super-block for both rows: scales are decoded once per
 // super-block with 32-bit SIMD masks (the utmp trick of ggml-cpu/quants.c:586-592), high nibbles are
 // used in place through an unsigned-by-signed dp4a on (q & 0xF0F0F0F0) followed by one >>4 of the sum,

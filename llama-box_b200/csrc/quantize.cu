@@ -1,4 +1,4 @@
-// quantize.cu — activation quantisation + RMS_NORM for the decode/prefill hot path (sm_100a).
+// quantize.cu — activation quantisation + RMS_NORM for the decode/prefill hot path (sm_90a).
 //
 // Replaces quantize_q8_1 (ggml-cuda/quantize.cu:4-48) and rms_norm_f32 (ggml-cuda/norm.cu:107-164),
 // but quantises the way the CPU oracle does so integer dot products are bit-identical:

@@ -1,4 +1,4 @@
-// rope.cu — ROPE, SET_ROWS (KV store) and their fused decode form (sm_100a).
+// rope.cu — ROPE, SET_ROWS (KV store) and their fused decode form (sm_90a).
 //
 // Replaces rope_norm / rope_neox (ggml-cuda/rope.cu:40-122,324-446), k_set_rows / k_set_rows_quant
 // (ggml-cuda/set-rows.cu:13-160) and quantize_f32_q8_0_block (cpy-utils.cuh:145-162).

@@ -13,7 +13,7 @@ WEIGHT_TYPES = (Q4_0, Q8_0, Q4_K, Q5_K, Q6_K)
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                      "(nvcc, sm_100a). llama-box_b200 has no CPU fallback.")
+                      "(nvcc, sm_90a). llama-box_b200 has no CPU fallback.")
 lib = C.CDLL(LIB_PATH)
 
 vp, i64, i32, f32 = C.c_void_p, C.c_int64, C.c_int, C.c_float

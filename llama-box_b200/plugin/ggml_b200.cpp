@@ -1,4 +1,4 @@
-// ggml_b200.cpp — the drop-in boundary: a ggml backend plug-in (libggml-b200.so) for NVIDIA B200.
+// ggml_b200.cpp — the drop-in boundary: a ggml backend plug-in (libggml-b200.so) for NVIDIA H100 (sm_90a).
 //
 // Exports exactly what ggml's registry binds when it dlopen()s a backend
 // (ggml/src/ggml-backend-impl.h:214-246, ggml/src/ggml-backend-reg.cpp:232-276):
@@ -8,8 +8,8 @@
 // name next to the executable, unchanged.  Everything that computes is a call into the kernel library's
 // C-ABI (include/b200_ops.h, include/b200_graph.h); this file only adapts ggml's structs.
 //
-// Compiled against the reference's own ggml headers (-I/root/reference/llama.cpp/ggml/{include,src}) with
-// -DGGML_MAX_NAME=128 to match llama-box (root CMakeLists.txt:62), linked against libggml-base.so.
+// Compiled against the reference's own ggml headers (staged in oracle/_ref/include by `make -C oracle ref`) with
+// -DGGML_MAX_NAME=128 to match llama-box (root CMakeLists.txt:62); libggml-base's symbols resolve against the host process.
 // Replaces ggml/src/ggml-cuda/ggml-cuda.cu's backend plumbing (:500-760 buffers, :2495-2600 streams/events,
 // :3138-3800 device/registry); nothing here is copied from it.
 #include "ggml.h"
@@ -551,12 +551,14 @@ static void * reg_proc(ggml_backend_reg_t, const char * name) {
     return nullptr;
 }
 
-static int count_blackwell(int * ids) {
+// devices the sm_90a kernels run on: compute capability 9.0 (H100 / H200)
+static int count_sm90(int * ids) {
     int n = 0, nd = 0;
     if (cudaGetDeviceCount(&nd) != cudaSuccess) { cudaGetLastError(); return 0; }
     for (int i = 0; i < nd && n < B200_MAX_DEVICES; i++) {
-        int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) { if (ids) ids[n] = i; n++; }
+        int major = 0, minor = 0;
+        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess &&
+            cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, i) == cudaSuccess && major == 9 && minor == 0) { if (ids) ids[n] = i; n++; }
     }
     return n;
 }
@@ -570,7 +572,7 @@ ggml_backend_reg_t ggml_backend_init(void) {
     static std::once_flag once;
     std::call_once(once, [] {
         int ids[B200_MAX_DEVICES];
-        g_ndev = count_blackwell(ids);
+        g_ndev = count_sm90(ids);
         for (int i = 0; i < g_ndev; i++) {
             b200_device_ctx & d = g_dev[i];
             cudaDeviceProp prop; cudaGetDeviceProperties(&prop, ids[i]);
@@ -584,5 +586,5 @@ ggml_backend_reg_t ggml_backend_init(void) {
     return &g_reg;
 }
 
-// 0 = "not usable here" (no sm_100 device): the registry then skips us (ggml-backend-reg.cpp:493-563)
-int ggml_backend_score(void) { return count_blackwell(nullptr) > 0 ? 100 : 0; }
+// 0 = "not usable here" (no sm_90 device): the registry then skips us (ggml-backend-reg.cpp:493-563)
+int ggml_backend_score(void) { return count_sm90(nullptr) > 0 ? 100 : 0; }

@@ -494,11 +494,11 @@ def test_glue_ops(b200):
     assert b200.lib.b200_kernel_launches() > 0
 
 
-# ------------------------------------------------------------------ a4: batched MUL_MAT on the tensor cores (tcgen05, mmq_tc.cu)
+# ------------------------------------------------------------------ a4: batched MUL_MAT on the tensor cores (wgmma, mmq_tc.cu)
 @pytest.mark.parametrize("t", [Q4_K, Q5_K, Q6_K])
 @pytest.mark.parametrize("m,k,n", [(128, 2048, 128), (256, 4096, 40), (48, 2048, 19), (384, 2048, 300), (1024, 4096, 512)])
 def test_mul_mat_q_tensor_core_vs_oracle(b200, t, m, k, n):
-    """the tcgen05 tile kernel against the C oracle (ggml_vec_dot_q*_K_q8_K restated): the integer sums are exact, so only the
+    """the wgmma tile kernel against the C oracle (ggml_vec_dot_q*_K_q8_K restated): the integer sums are exact, so only the
     f32 summation order over super-blocks differs — same bound as the matvec"""
     rng = np.random.default_rng(1000 + m + n)
     W = rand_blocks(rng, t, m, k)
@@ -599,7 +599,7 @@ def test_fused_decode_attention_vs_oracle_at_depth(b200, kvt, hd, nh, nhkv):
 @pytest.mark.parametrize("kvt", [F16, Q8_0])
 @pytest.mark.parametrize("nh,nhkv,nt,nkv,past", [(8, 2, 128, 256, 100), (4, 4, 200, 768, 512), (32, 8, 512, 1024, 512), (8, 1, 33, 512, 300), (4, 2, 512, 4096, 3584)])
 def test_flash_attn_tensor_core(b200, kvt, nh, nhkv, nt, nkv, past):
-    """prefill-shaped FLASH_ATTN_EXT (>= 16 tokens, head 128): tcgen05 S = Q K^T and O = P V with f16 operands, f32 softmax.
+    """prefill-shaped FLASH_ATTN_EXT (>= 16 tokens, head 128): wgmma S = Q K^T and O = P V with f16 operands, f32 softmax.
     Checked against an f64 evaluation of the same attention on the cache's own (f16-rounded / de-quantised) K, V and the f16-rounded
     Q; f16 P and f16 d*q de-quantisation bound the deviation to ~1e-3 relative (the reference's CUDA path rounds the same way);
     the CPU oracle (f32 P; fp16 accumulation for F16 V) must agree to its own accuracy.  Causal mask with `past` cached positions,

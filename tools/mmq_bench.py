@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Kernel-level timing of the batched MUL_MAT (b200_mul_mat_q, tcgen05 path) on the Llama-3-8B matmul shapes at a 512-token
+"""Kernel-level timing of the batched MUL_MAT (b200_mul_mat_q, wgmma path) on the Llama-3-8B matmul shapes at a 512-token
 ubatch: CUDA events on the launching stream, 20 repetitions after 3 warm-ups, weights of all shapes (> L2) cycled between reps."""
 import json
 import os

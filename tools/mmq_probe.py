@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Bring-up aid for the tcgen05 batched MUL_MAT (mmq_tc.cu): one shape, error statistics against the C oracle, sample values."""
+"""Bring-up aid for the wgmma batched MUL_MAT (mmq_tc.cu): one shape, error statistics against the C oracle, sample values."""
 import os
 import sys
 

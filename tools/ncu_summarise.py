@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Turn the round's `ncu --set full` captures (gpurun_out/r2_*.ncu-rep, produced by tools/profile_r2.sh on a B200) into the
-committed evidence under profiles/: one TSV per capture with the metrics the roofline discussion uses, the launch-list summary,
+"""Turn the round's `ncu --set full` captures (r2_*.ncu-rep, produced by tools/profile_r2.sh on the GPU) into the
+evidence under profiles/ (git-ignored, per machine): one TSV per capture with the metrics the roofline discussion uses, the launch-list summary,
 and profiles/r2_kernel_traffic.json (DRAM bytes per algorithmic byte of the matvec launches — what bench.py's roofline.traffic
 reads instead of a hard-coded constant).  Runs here (no GPU): `ncu -i <rep> --page raw --csv`."""
 import csv

@@ -15,10 +15,10 @@ $NCU --set full --import-source on -k regex:fattn_vec -s 40 -c 2 -f -o /tmp/prof
 # 3. --set full: the matvec launches of one layer in situ (QKV, wo, gate/up, down), the lm_head launch (persistent kernel) and argmax
 $NCU --set full --import-source on -k regex:mmvq_kernel -s 64 -c 8 -f -o /tmp/prof/r2_mmvq $B --steps 2 --warmup 2 > /dev/null 2>&1
 $NCU --set full --import-source on -k regex:'mk_kernel|argmax' -s 2 -c 2 -f -o /tmp/prof/r2_lmhead_argmax $B --steps 2 --warmup 2 > /dev/null 2>&1
-# 4. --set full: the tcgen05 prefill GEMM (ffn_up shape 14336 x 4096, 512 tokens) + its activation quantiser
+# 4. --set full: the wgmma prefill GEMM (ffn_up shape 14336 x 4096, 512 tokens) + its activation quantiser
 $NCU --set full --import-source on -k regex:'mmq_tc|quantize_mmq' -c 4 -f -o /tmp/prof/r2_mmq_tc python tools/mmq_probe.py q4_K 14336 4096 512 > gpurun_out/r2_mmq_tc_probe.log 2>&1
 $NCU --set full --import-source on -k regex:'mmq_tc' -c 1 -f -o /tmp/prof/r2_mmq_tc_q6k python tools/mmq_probe.py q6_K 4096 14336 512 >> gpurun_out/r2_mmq_tc_probe.log 2>&1
-# 5. --set full: the tcgen05 multi-token attention (32 heads / 8 KV heads, 512-token ubatch at depth 3584 -> n_kv 4096), F16 and Q8_0 cache
+# 5. --set full: the wgmma multi-token attention (32 heads / 8 KV heads, 512-token ubatch at depth 3584 -> n_kv 4096), F16 and Q8_0 cache
 $NCU --set full --import-source on -k regex:fattn_tc -c 1 -f -o /tmp/prof/r2_fattn_tc_f16 python tools/fattn_probe.py f16 32 8 512 4096 3584 > gpurun_out/r2_fattn_tc_probe.log 2>&1
 $NCU --set full --import-source on -k regex:fattn_tc -c 1 -f -o /tmp/prof/r2_fattn_tc_q8 python tools/fattn_probe.py q8_0 32 8 512 4096 3584 >> gpurun_out/r2_fattn_tc_probe.log 2>&1
 ls -la /tmp/prof/*.ncu-rep

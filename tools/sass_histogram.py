@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """SASS opcode histogram per kernel of libb200ops.so (cuobjdump -sass), written to profiles/<round>_sass_opcodes.txt.
-Evidence for what the kernels are made of: UTCHMMA / LDTM (tcgen05 + TMEM), UBLKCP / SYNCS (TMA bulk copies + mbarriers),
+Evidence for what the kernels are made of: HGMMA (wgmma), UBLKCP / SYNCS (TMA bulk copies + mbarriers),
 IDP.4A (dp4a) ... — the PTX names never appear in SASS (B200_PROFILING.md)."""
 import collections
 import os
@@ -24,9 +24,9 @@ for ln in txt.splitlines():
     m = re.match(r"\s*/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_]*(?:\.[A-Z0-9_]+)*)", ln)
     if m and kern:
         hist[kern][m.group(1)] += 1
-KEY = ("UTCHMMA", "UTCIMMA", "UTCQMMA", "LDTM", "STTM", "UTCBAR", "UTCATOMSWS", "UBLKCP", "UTMALDG", "SYNCS", "IDP", "HFMA2", "HMUL2", "HADD2", "FFMA", "LDG", "LDS", "STS", "STG", "SHFL", "BAR", "MUFU", "DFMA", "DADD")
+KEY = ("HGMMA", "UTCHMMA", "UTCIMMA", "UTCQMMA", "LDTM", "STTM", "UTCBAR", "UTCATOMSWS", "UBLKCP", "UTMALDG", "SYNCS", "IDP", "HFMA2", "HMUL2", "HADD2", "FFMA", "LDG", "LDS", "STS", "STG", "SHFL", "BAR", "MUFU", "DFMA", "DADD")
 with open(out, "w") as f:
-    f.write("# SASS opcode histogram per kernel of llama-box_b200/libb200ops.so (cuobjdump -sass, sm_100a); tools/sass_histogram.py\n")
+    f.write("# SASS opcode histogram per kernel of llama-box_b200/libb200ops.so (cuobjdump -sass, sm_90a); tools/sass_histogram.py\n")
     f.write("# columns: total instructions | selected opcode families (prefix match)\n")
     agg = collections.defaultdict(collections.Counter)
     for k, c in hist.items():
