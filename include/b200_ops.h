@@ -302,8 +302,8 @@ B200_API int b200_rope_kv_store2(const float *q_src, float *q_dst, const float *
  *   k,v  cache rows of kv_type (F16 or Q8_0): (pos, kv_head) at base + pos*row_stride + kv_head*head_stride (bytes)
  *   mask f16 [n_tok_padded][n_kv] (row stride mask_row_stride halves) or NULL; -inf = masked
  *   dst  f32 [n_tok][n_head][dv] contiguous
- *   workspace: b200_flash_attn_workspace(...) bytes for split-KV partials + completion counters; zero it ONCE
- *   (the counters reset themselves at the end of every launch) */
+ *   workspace: b200_flash_attn_workspace(...) bytes, now always 0: the KV splits merge inside a thread-block cluster;
+ *   the argument is ignored and may be NULL */
 B200_API int64_t b200_flash_attn_workspace(int64_t dv, int64_t n_head, int64_t n_tok, int64_t n_kv);
 B200_API int b200_flash_attn_ext(const float *q, int64_t q_tok_stride, int64_t q_head_stride,
                                  const void *k, int64_t k_row_stride, int64_t k_head_stride,

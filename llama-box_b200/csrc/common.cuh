@@ -29,6 +29,18 @@ inline cudaError_t b200_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block
     cfg.attrs = at; cfg.numAttrs = b200_pdl_enabled() ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
+// ... as thread-block clusters of cluster_x CTAs along grid.x (grid.x must be a multiple of cluster_x; more than 8 needs the
+// kernel's cudaFuncAttributeNonPortableClusterSizeAllowed)
+template <typename... KArgs, typename... Args>
+inline cudaError_t b200_launch_pdl_cluster(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, unsigned cluster_x, Args &&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute at[2];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = cluster_x; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = b200_pdl_enabled() ? 2 : 1;
+    return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
 #endif
 
 #define B200_CUDA(expr) do { int _s = b200_check((expr), #expr); if (_s != B200_OK) return _s; } while (0)
@@ -157,6 +169,19 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void * gsrc, uint32_t byt
 // programmatic dependent launch (guide G9): overlap this kernel's prologue with the previous tail
 __device__ __forceinline__ void pdl_wait()    { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// thread-block cluster: hardware barrier over every thread of the cluster (all threads of each warp must take part), and loads from
+// a peer CTA's shared memory (distributed shared memory)
+__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait_acquire()   { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait()           { asm volatile("barrier.cluster.wait.aligned;" ::: "memory"); }
+__device__ __forceinline__ uint32_t cluster_map(const void * smem_p, uint32_t rank) {
+    uint32_t a; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(smem_p)), "r"(rank)); return a;
+}
+__device__ __forceinline__ float ld_cluster_f32(uint32_t addr) {
+    float v; asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory"); return v;
+}
 
 // ---- B200_TRACE=1: in-kernel timeline of the decode chain (tools/trace_decode.py).  A traced CTA claims a record with one atomic
 // and stamps %globaltimer at entry / exit plus clock64 at the points in between; records are read back per source file.

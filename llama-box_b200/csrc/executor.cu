@@ -272,7 +272,7 @@ struct GraphEntry { cudaGraphExec_t exec = nullptr; int64_t kernels = 0; uint64_
 
 struct b200_executor {
     int device = 0;
-    // workspace: [act q8_K][act q8_0][fattn partials]
+    // workspace: [act q8_K][act q8_0][attention: persistent-kernel split merge | decode q|k|v scratch | rope table]
     uint8_t * ws = nullptr; size_t ws_bytes = 0;
     size_t off_act[2] = {0, 0}, act_bytes[2] = {0, 0}, off_fa = 0, fa_bytes = 0;
     uint64_t act_id[2] = {0, 0}; const void * act_ptr[2] = {nullptr, nullptr}; int64_t act_cols[2] = {0, 0};
@@ -291,6 +291,11 @@ struct b200_executor {
 };
 
 namespace {
+
+// the persistent kernel's attention phase (decode_mk.cu) merges its KV splits through global memory: 256 KiB of completion
+// counters (zeroed once, self-cleaning), then up to 64 splits of (hd + 2)-float rows per head.  The attention launch itself
+// (fattn.cu) merges inside a thread-block cluster and needs none of it.
+static size_t mk_attn_ws_bytes(int64_t hd, int64_t nh) { return 256 * 1024 + (size_t)64 * nh * (hd + 2) * 4; }
 
 // a kernel launch — or, in a dry run, just its count
 #define KL(call) (dry ? (plan_note(#call), (int)B200_OK) : (int)(call))
@@ -616,7 +621,7 @@ struct Runner {
         if ((p.mode & ~2) || p.n_dims > hd || p.n_dims % 8 != 0 || (p.mode == 2 && p.n_dims % 16 != 0)) return false;
         const b200_node & F = nodes[fa];
         // executor scratch behind the attention workspace: q | k | v projections of this token
-        const size_t fa_ws = (size_t)b200_flash_attn_workspace(hd, nh, 1, F.src[1].ne[1]);
+        const size_t fa_ws = mk_attn_ws_bytes(hd, nh);
         if (!dry && (((fa_ws + 255) & ~(size_t)255) + (size_t)(nh + 2 * nhk) * hd * 4 + 1024 > ex->fa_bytes)) return false;
         float * sq = dry ? (float *)(uintptr_t)0x10000 : (float *)(ex->ws + ex->off_fa + ((fa_ws + 255) & ~(size_t)255));
         float * skn = sq + nh * hd, * svn = skn + nhk * hd;
@@ -1015,7 +1020,7 @@ int plan_workspace(b200_executor * ex, const b200_node * nodes, int n) {
             for (int kd = 0; kd < 2; kd++) { const size_t b = (size_t)(8 * act_col_bytes(kd, (nd.src[0].ne[0] + 255) / 256 * 256)); if (b > act[kd]) act[kd] = b; }
         } else if (nd.op == B200_OP_FLASH_ATTN_EXT) {
             size_t b = (size_t)b200_flash_attn_workspace(nd.src[2].ne[0], nd.src[0].ne[2], nd.src[0].ne[1], nd.src[1].ne[1]);
-            if (nd.src[0].ne[1] == 1) b = ((b + 255) & ~(size_t)255) + (size_t)(nd.src[0].ne[2] + 2 * nd.src[1].ne[2]) * nd.src[0].ne[0] * 4 + 512;   // + q|k|v scratch of try_attn_block
+            if (nd.src[0].ne[1] == 1) b = mk_attn_ws_bytes(nd.src[0].ne[0], nd.src[0].ne[2]) + (size_t)(nd.src[0].ne[2] + 2 * nd.src[1].ne[2]) * nd.src[0].ne[0] * 4 + 512;   // + q|k|v scratch of try_attn_block
             b = ((b + 255) & ~(size_t)255) + 1024;                // + the per-token rope table (last KiB of the region)
             if (b > fa) fa = b;
         }
@@ -1029,7 +1034,7 @@ int plan_workspace(b200_executor * ex, const b200_node * nodes, int n) {
     for (auto & g : ex->graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
     ex->graphs.clear();
     if (ex->ws) { cudaDeviceSynchronize(); cudaFree(ex->ws); ex->ws = nullptr; }
-    if (cudaMalloc((void **)&ex->ws, total) != cudaSuccess || cudaMemset(ex->ws, 0, total) != cudaSuccess) {   /* zeroed once: flash-attn split counters */ cudaGetLastError(); b200_set_error("executor: cannot allocate %zu bytes of workspace", total); return B200_ERR_CUDA; }
+    if (cudaMalloc((void **)&ex->ws, total) != cudaSuccess || cudaMemset(ex->ws, 0, total) != cudaSuccess) {   /* zeroed once: the persistent kernel's split counters */ cudaGetLastError(); b200_set_error("executor: cannot allocate %zu bytes of workspace", total); return B200_ERR_CUDA; }
     ex->ws_bytes = total;
     ex->off_act[0] = 0; ex->off_act[1] = up(act[0]); ex->off_fa = up(act[0]) + up(act[1]);
     ex->act_bytes[0] = act[0]; ex->act_bytes[1] = act[1]; ex->fa_bytes = fa;

@@ -8,10 +8,10 @@
 // oracle accumulates in fp16; we accumulate in f32, which is strictly more accurate.)
 //
 // Mapping: D/8 lanes per KV position (8 elements = one 16-byte load per lane for F16), so a warp
-// streams 2 (D=128) or 4 (D=64) positions per step with fully coalesced rows; up to 4 query heads of
-// one GQA group share every K/V load; KV is split over CTAs (grid.x) to fill the SMs (132 on an H100), each split
-// writes (m, l, acc) partials that a second kernel merges.  HBM-bound: bytes = K+V rows once per
-// head tile.
+// streams 2 (D=128) or 4 (D=64) positions per step with fully coalesced rows; up to 2 query heads of
+// one GQA group share every K/V load; KV is split over the CTAs of a thread-block cluster (grid.x) to fill the SMs (132 on
+// an H100), and the cluster merges the splits' (m, l, acc) partials through distributed shared memory.  HBM-bound: bytes =
+// K+V rows once per head tile.
 #include "common.cuh"
 #include "ropeutil.cuh"
 #include <math.h>
@@ -22,7 +22,7 @@
 #ifndef FA_MIN_CTAS
 #define FA_MIN_CTAS 1      // (4 = at most 128 registers, so that a CTA fits next to a resident matvec CTA: measured no gain)
 #endif
-#define FA_MAX_SPLITS 64
+#define FA_MAX_CLUSTER 16  // KV splits of one (token, head tile) = CTAs of one cluster
 
 B200_TRACE_DECL(g_fa_trace)
 
@@ -50,7 +50,7 @@ __device__ __forceinline__ void load_q80_8(const uint8_t * row, int dl, int (&q)
 struct FaFuse {
     const float * q_src; float * q_dst; const float * k_new; const float * v_new;
     const int32_t * pos; const float * ff; const int64_t * k_ids; const int64_t * v_ids;
-    RopeDev rp; int enabled; int early_trigger;
+    RopeDev rp; int enabled;
     // cos/sin table of this token: the same for every layer, so the first attention launch of a token computes it (every CTA for
     // itself, one CTA also stores it) and the other layers just load 512 bytes: tab_mode 0 = compute (+ store if rope_tab), 1 = load
     float * rope_tab; int tab_mode;
@@ -109,13 +109,16 @@ __device__ __forceinline__ void lds_q80_8(const uint8_t * row, int dl, int (&q)[
 // LEAN = 1: the decode instance of layers 1..n-1 — fused rope / KV store with the cos/sin table loaded (tab_mode 1), a mask, no ALiBi,
 // no soft-cap: the switches below become constants and powf / tanhf / the table computation (sincosf, YaRN) leave the kernel.  These
 // launches last ~10 us and start with a cold instruction cache, so the size of the code they step through is their critical path.
+//
+// The splits of one (token, head tile) are one thread-block cluster along grid.x (cluster rank = split).  Each CTA leaves its split's
+// (m, l) per head and its G x D accumulator in shared memory; after a cluster barrier CTA r merges a 1/C slice of the tile's output,
+// reading every peer's partials through distributed shared memory in rank order 0..C-1 (so the result does not depend on timing).
 template <int D, int KVT, int G, int LEAN = 0>
 __global__ void __launch_bounds__(FA_WARPS * 32, FA_MIN_CTAS) fattn_vec_kernel(
         const float * __restrict__ q, int64_t q_ts, int64_t q_hs,
         const uint8_t * __restrict__ kc, int64_t k_rs, int64_t k_hs,
         const uint8_t * __restrict__ vc, int64_t v_rs, int64_t v_hs,
-        const uint16_t * __restrict__ mask, int64_t mask_rs,
-        float * __restrict__ dst, float * __restrict__ ws, unsigned int * __restrict__ counters,
+        const uint16_t * __restrict__ mask, int64_t mask_rs, float * __restrict__ dst,
         int n_head, int n_head_kv, int n_kv, int split_len, int n_splits,
         float scale, float max_bias_rt, float softcap_rt, float m0, float m1, int nh_log2, const FaFuse fu) {
     const float max_bias = LEAN ? 0.0f : max_bias_rt, softcap = LEAN ? 0.0f : softcap_rt;
@@ -132,13 +135,11 @@ __global__ void __launch_bounds__(FA_WARPS * 32, FA_MIN_CTAS) fattn_vec_kernel(
     __shared__ __align__(16) uint8_t s_newk[D * 2 + 32], s_newv[D * 2 + 32];
     constexpr int MAXIT = 4;
     constexpr int pstride = FA_WARPS * PPW;
+    constexpr int CH = pstride * MAXIT;                 // positions of one chunk (MAXIT per lane group)
     const int p_begin = split * split_len;
     const int p_end   = min(n_kv, p_begin + split_len);
     const int base0 = p_begin + warp * PPW + sg;
-    // K / V of the first chunk of this split.  On the decode path (fu.enabled) the cells of EARLIER tokens were written by earlier
-    // launches of the token loop, and pos / cell ids are graph inputs: all of it may be fetched before griddepcontrol.wait, while
-    // the previous kernel (the QKV projection) is still running — a memory round trip off the token's critical path.
-    uint4 kpre[MAXIT], vpre[MAXIT]; float kdpre[MAXIT], vdpre[MAXIT];
+    const uint16_t * mrow = (LEAN || mask) ? mask + (int64_t)tok * mask_rs : nullptr;
     int kcell = -1, vcell = -1, tok_pos = 0;
     B200_TRACE_OPEN(g_fa_trace, fu.trace && threadIdx.x == 0 && tok == 0 && ((split == 0 && tile == 0) || (split == n_splits - 1 && tile == (int)gridDim.y - 1)), tr)
     if (tr) { tr[8] = ((unsigned long long)split << 48) | ((unsigned long long)(unsigned)n_kv << 16) | (unsigned)n_splits; tr[9] = 0; }
@@ -152,19 +153,45 @@ __global__ void __launch_bounds__(FA_WARPS * 32, FA_MIN_CTAS) fattn_vec_kernel(
             load_q80_8(vrow, dl, q2, vd); vr = make_uint4((uint32_t)q2[0], (uint32_t)q2[1], 0, 0);
         }
     };
-    if (fused) {
-        kcell = (int)fu.k_ids[0]; vcell = (int)fu.v_ids[0]; tok_pos = fu.pos[0];
+    // mask of this lane group's positions in the chunk at `base`: -inf beyond the split
+    auto load_mask = [&](int base, float (&m)[MAXIT]) {
 #pragma unroll
         for (int it = 0; it < MAXIT; it++) {
-            const int p = base0 + it * pstride;
-            kpre[it] = make_uint4(0, 0, 0, 0); vpre[it] = kpre[it]; kdpre[it] = 0.0f; vdpre[it] = 0.0f;
-            if (p < p_end) load_kv(p, kpre[it], vpre[it], kdpre[it], vdpre[it]);
+            const int p = base + it * pstride;
+            m[it] = p < p_end ? ((LEAN || mrow) ? h2f(__ldg(mrow + p)) : 0.0f) : -INFINITY;
         }
+    };
+    // K / V of the chunk at `base`; no load for a position that cannot contribute (beyond the split, or masked without ALiBi)
+    auto load_chunk = [&](int base, const float (&m)[MAXIT], uint4 (&kr)[MAXIT], uint4 (&vr)[MAXIT], float (&kd)[MAXIT], float (&vd)[MAXIT]) {
+#pragma unroll
+        for (int it = 0; it < MAXIT; it++) {
+            const int p = base + it * pstride;
+            kr[it] = make_uint4(0, 0, 0, 0); vr[it] = kr[it]; kd[it] = 0.0f; vd[it] = 0.0f;
+            if (p < p_end && !(m[it] == -INFINITY && max_bias <= 0.0f)) load_kv(p, kr[it], vr[it], kd[it], vd[it]);
+        }
+    };
+    // the chunk being computed (mask, K, V) and the next chunk's mask
+    float mcur[MAXIT], mnext[MAXIT]; uint4 kcur[MAXIT], vcur[MAXIT]; float kdcur[MAXIT], vdcur[MAXIT];
+    // First chunk.  On the decode path (fu.enabled) the cells of EARLIER tokens were written by earlier launches of the token loop, and
+    // pos / cell ids are graph inputs: all of it may be fetched before griddepcontrol.wait, while the previous kernel (the QKV projection)
+    // is still running — a memory round trip off the token's critical path.  The mask is read that early only by the layers after the
+    // first (LEAN): whatever produces it ran launches ago, and fully masked positions then cost no K / V traffic either.
+    if (fused) {
+        kcell = (int)fu.k_ids[0]; vcell = (int)fu.v_ids[0]; tok_pos = fu.pos[0];
+        if (LEAN) { load_mask(base0, mcur); load_mask(base0 + CH, mnext); }
+        else {
+#pragma unroll
+            for (int it = 0; it < MAXIT; it++) mcur[it] = 0.0f;       // not known yet: load every position of the split
+        }
+        load_chunk(base0, mcur, kcur, vcur, kdcur, vdcur);
     }
     B200_TRACE_AT(tr, 2);                     // first K / V chunk requested
-    if (fu.early_trigger == 1) pdl_trigger(); // B200_FA_EARLY_TRIGGER=1: the next kernel may prime its weight ring during the attention — measured slower (its burst delays our loads)
     pdl_wait();
     B200_TRACE_AT(tr, 3);                     // QKV projection complete
+    if (!LEAN) {
+        load_mask(base0, mcur); load_mask(base0 + CH, mnext);
+        if (!fused) load_chunk(base0, mcur, kcur, vcur, kdcur, vdcur);
+    }
     float qraw[G][8], qpar[G][8];
     if (fused) {
         // this token's query heads: issue the loads now, rope them once the table is in shared memory
@@ -251,32 +278,28 @@ __global__ void __launch_bounds__(FA_WARPS * 32, FA_MIN_CTAS) fattn_vec_kernel(
         for (int e = 0; e < 8; e++) acc[g][e] = 0.0f; }
 
     const unsigned gmask = ((1u << LP) - 1u) << (sg * LP);   // lanes sharing one KV position (converged inside the loop)
-    const uint16_t * mrow = (LEAN || mask) ? mask + (int64_t)tok * mask_rs : nullptr;
 
-    // positions are visited in chunks of MAXIT per lane group: every load of a chunk (mask, K, V) is issued before any
-    // arithmetic, so a chunk costs one memory round trip instead of MAXIT (decode attention is latency-bound: a split is
-    // a few dozen positions).  K/V of masked positions are loaded but never used.
-    for (int base = base0; base < p_end; base += pstride * MAXIT) {
-        float mraw[MAXIT]; uint4 kraw[MAXIT], vraw[MAXIT]; float kdv[MAXIT], vdv[MAXIT];
-        const bool pre = fused && base == base0;          // first chunk: K / V already in registers
+    // positions are visited in chunks of MAXIT per lane group.  Every load of a chunk is issued before any arithmetic on it, and the
+    // next chunk's K / V (and the mask of the one after) are issued before this chunk's arithmetic: a split of several chunks pays about
+    // one memory round trip, not one per chunk (decode attention is latency-bound).
+    for (int base = base0; base < p_end; base += CH) {
+        if (fused) {
 #pragma unroll
-        for (int it = 0; it < MAXIT; it++) {
-            const int p = base + it * pstride;
-            mraw[it] = -INFINITY; kraw[it] = make_uint4(0, 0, 0, 0); vraw[it] = kraw[it]; kdv[it] = 0.0f; vdv[it] = 0.0f;
-            if (p < p_end) {
-                mraw[it] = (LEAN || mrow) ? h2f(__ldg(mrow + p)) : 0.0f;
-                if (pre) { kraw[it] = kpre[it]; vraw[it] = vpre[it]; kdv[it] = kdpre[it]; vdv[it] = vdpre[it]; }
-                else load_kv(p, kraw[it], vraw[it], kdv[it], vdv[it]);
+            for (int it = 0; it < MAXIT; it++) {
+                const int p = base + it * pstride;
                 if (p == kcell) {                               // this token's own cell: from shared memory (the global cell is being written by another CTA)
-                    if (KVT == B200_TYPE_F16) kraw[it] = *(const uint4 *)(s_newk + dl * 16);
-                    else { int q2[2]; lds_q80_8(s_newk, dl, q2, kdv[it]); kraw[it].x = (uint32_t)q2[0]; kraw[it].y = (uint32_t)q2[1]; }
+                    if (KVT == B200_TYPE_F16) kcur[it] = *(const uint4 *)(s_newk + dl * 16);
+                    else { int q2[2]; lds_q80_8(s_newk, dl, q2, kdcur[it]); kcur[it].x = (uint32_t)q2[0]; kcur[it].y = (uint32_t)q2[1]; }
                 }
                 if (p == vcell) {
-                    if (KVT == B200_TYPE_F16) vraw[it] = *(const uint4 *)(s_newv + dl * 16);
-                    else { int q2[2]; lds_q80_8(s_newv, dl, q2, vdv[it]); vraw[it].x = (uint32_t)q2[0]; vraw[it].y = (uint32_t)q2[1]; }
+                    if (KVT == B200_TYPE_F16) vcur[it] = *(const uint4 *)(s_newv + dl * 16);
+                    else { int q2[2]; lds_q80_8(s_newv, dl, q2, vdcur[it]); vcur[it].x = (uint32_t)q2[0]; vcur[it].y = (uint32_t)q2[1]; }
                 }
             }
         }
+        float mnn[MAXIT]; uint4 knext[MAXIT], vnext[MAXIT]; float kdnext[MAXIT], vdnext[MAXIT];
+        load_chunk(base + CH, mnext, knext, vnext, kdnext, vdnext);
+        load_mask(base + 2 * CH, mnn);
         // one position per lane group and step.  The decode instance keeps this loop ROLLED (the K / V registers rotate through
         // slot 0): unrolled it is 20 KB of straight-line code that every launch fetches cold, rolled it is 5 KB fetched once
         auto step = [&](const float mr, const uint4 & kr, const uint4 & vr, const float kd, const float vd) {
@@ -329,26 +352,31 @@ __global__ void __launch_bounds__(FA_WARPS * 32, FA_MIN_CTAS) fattn_vec_kernel(
         if constexpr (LEAN) {
 #pragma unroll 1
             for (int it = 0; it < MAXIT; it++) {
-                const float mr = mraw[0]; const uint4 kr = kraw[0], vr = vraw[0]; const float kd = kdv[0], vd = vdv[0];
+                const float mr = mcur[0]; const uint4 kr = kcur[0], vr = vcur[0]; const float kd = kdcur[0], vd = vdcur[0];
 #pragma unroll
-                for (int j = 0; j + 1 < MAXIT; j++) { mraw[j] = mraw[j + 1]; kraw[j] = kraw[j + 1]; vraw[j] = vraw[j + 1]; kdv[j] = kdv[j + 1]; vdv[j] = vdv[j + 1]; }
-                if (mr == -INFINITY || base + it * pstride >= p_end) continue;      // masked, or beyond the split (uniform inside the LP-lane group)
+                for (int j = 0; j + 1 < MAXIT; j++) { mcur[j] = mcur[j + 1]; kcur[j] = kcur[j + 1]; vcur[j] = vcur[j + 1]; kdcur[j] = kdcur[j + 1]; vdcur[j] = vdcur[j + 1]; }
+                if (mr == -INFINITY) continue;      // masked, or beyond the split (uniform inside the LP-lane group)
                 step(mr, kr, vr, kd, vd);
             }
         } else {
 #pragma unroll
             for (int it = 0; it < MAXIT; it++) {
-                if (mraw[it] == -INFINITY && max_bias <= 0.0f) continue;       // masked, or beyond the split (uniform inside the LP-lane group)
+                if (mcur[it] == -INFINITY && max_bias <= 0.0f) continue;       // masked, or beyond the split (uniform inside the LP-lane group)
                 if (base + it * pstride >= p_end) continue;
-                step(mraw[it], kraw[it], vraw[it], kdv[it], vdv[it]);
+                step(mcur[it], kcur[it], vcur[it], kdcur[it], vdcur[it]);
             }
+        }
+#pragma unroll
+        for (int it = 0; it < MAXIT; it++) {
+            mcur[it] = mnext[it]; kcur[it] = knext[it]; vcur[it] = vnext[it]; kdcur[it] = kdnext[it]; vdcur[it] = vdnext[it]; mnext[it] = mnn[it];
         }
     }
 
     B200_TRACE_AT(tr, 5);                     // positions of this split done (warp 0)
-    // ---- merge the PPW position groups of the warp, then the warps, then write ------------------
+    // ---- merge the PPW position groups of the warp, then the warps: this split's partial, in shared memory ----------------
     __shared__ float sM[FA_WARPS][G], sL[FA_WARPS][G];
     __shared__ float sA[FA_WARPS][G][D];
+    __shared__ float cM[G], cL[G], cA[G][D];            // the split's partial, read by every CTA of the cluster
 #pragma unroll
     for (int g = 0; g < G; g++) {
 #pragma unroll
@@ -378,132 +406,77 @@ __global__ void __launch_bounds__(FA_WARPS * 32, FA_MIN_CTAS) fattn_vec_kernel(
             const float sc = sM[w][g] == -INFINITY ? 0.0f : expf(sM[w][g] - Mn);
             a += sA[w][g][e] * sc; l += sL[w][g] * sc;
         }
-        const int h = h0 + g;
-        if (n_splits == 1) {
-            dst[((int64_t)tok * n_head + h) * D + e] = a * (1.0f / l);            // ops.cpp:8390-8392
-        } else {
-            float * wp = ws + (((int64_t)split * gridDim.z + tok) * n_head + h) * (D + 4);     // rows of D + 4 floats: 16-byte aligned for the merge
-            wp[e] = a;
-            if (e == 0) { wp[D] = Mn; wp[D + 1] = l; }
-        }
+        cA[g][e] = a;
+        if (e == 0) { cM[g] = Mn; cL[g] = l; }
     }
-    if (n_splits > 1) {
-        // the last CTA of this (token, head tile) to finish merges all splits (replaces the separate
-        // flash_attn_combine_results launch, fattn-common.cuh:645-701); the counter cleans itself for the next launch
-        __shared__ unsigned int s_last;
-        __syncthreads();                      // every thread's partials are ordered before thread 0's fence (the cooperative-groups grid.sync pattern)
-        if (threadIdx.x == 0) {
-            asm volatile("fence.acq_rel.gpu;" ::: "memory");       // (__threadfence() is the sequentially-consistent MEMBAR.SC)
-            const unsigned int prev = atomicAdd(&counters[tok * gridDim.y + tile], 1u);
-            s_last = prev == (unsigned int)(n_splits - 1);
-            if (s_last) counters[tok * gridDim.y + tile] = 0;
-        }
-        __syncthreads();
-        B200_TRACE_AT(tr, 6);                 // partials written, completion counted
-        // every CTA has now either exited or reached this point: let the next kernel (the wo projection) launch and prime its weight
-        // ring while the 8 merging CTAs finish — its griddepcontrol.wait still waits for the whole grid (B200_FA_EARLY_TRIGGER=2)
-        if (fu.early_trigger == 2) pdl_trigger();
-        if (s_last) {
-            if (tr) tr[9] = 1;
-            asm volatile("fence.acq_rel.gpu;" ::: "memory");
-            // The partial accumulators do not depend on the scale factors: request the first half of them (one float4 per thread and
-            // split — G * D / 4 = 128 items for D = 128) together with the (m, l) pairs, so that the merge costs two memory round trips
-            // instead of one per 8 splits and output (it was 9 us of a 17 us launch at 24 splits)
-            __shared__ float s_sc[FA_MAX_SPLITS][G];
-            __shared__ float s_l[FA_MAX_SPLITS][G];
-            __shared__ float s_m2[FA_MAX_SPLITS][G];
-            const int n_rows = gridDim.z * n_head;
-            constexpr int NB = 12;                                  // splits per batch of loads; the batch loop stays rolled (code size)
-            constexpr int items = G * D / 4;
-            const int64_t sstride = (int64_t)n_rows * (D + 4) / 4;    // float4 units between the same row of consecutive splits
-            const int it0 = threadIdx.x;
-            const bool have0 = it0 < items;
-            const int g0 = it0 / (D / 4), e0 = it0 % (D / 4);
-            const float4 * src0 = (const float4 *)(ws + (int64_t)(tok * n_head + h0 + g0) * (D + 4)) + e0;
-            float4 v[NB];
+    // ---- merge the splits over the cluster (replaces flash_attn_combine_results, fattn-common.cuh:645-701) ----------------
+    cluster_arrive_release();                 // this split's partial is published to the cluster
+    pdl_trigger();                            // the next kernel (the wo projection) may launch; its griddepcontrol.wait still waits for this grid
+    cluster_wait_acquire();
+    B200_TRACE_AT(tr, 6);                     // every split of the tile published
+    // CTA `split` writes outputs [split * per, (split + 1) * per) of the tile's G x D; every peer's loads are issued before any is used
+    const int per = (G * D + n_splits - 1) / n_splits;
+    const int i_end = min(G * D, (split + 1) * per);
+    for (int idx = split * per + (int)threadIdx.x; idx < i_end; idx += FA_WARPS * 32) {
+        const int g = idx / D, e = idx % D;
+        float pm[FA_MAX_CLUSTER], pl[FA_MAX_CLUSTER], pa[FA_MAX_CLUSTER];
 #pragma unroll
-            for (int j = 0; j < NB; j++) { v[j] = make_float4(0, 0, 0, 0); if (have0 && j < n_splits) v[j] = __ldcg(src0 + j * sstride); }
-            for (int idx = threadIdx.x; idx < n_splits * G; idx += FA_WARPS * 32) {
-                const int sp = idx / G, g = idx % G;
-                const float2 ml = __ldcg((const float2 *)(ws + ((int64_t)sp * n_rows + tok * n_head + h0 + g) * (D + 4) + D));   // every (m, l) pair in one round trip
-                s_sc[sp][g] = ml.x; s_l[sp][g] = ml.y;
-            }
-            __syncthreads();
-            // scale factors: one (split, head) per thread, each finding its head's maximum itself (independent broadcast LDS) — a serial
-            // loop of one thread per head over the splits cost 1 us
-            for (int idx = threadIdx.x; idx < n_splits * G; idx += FA_WARPS * 32) {
-                const int sp = idx / G, g = idx % G;
-                float Mn = -INFINITY;
-                for (int q = 0; q < n_splits; q++) Mn = fmaxf(Mn, s_sc[q][g]);
-                const float m = s_sc[sp][g];
-                s_m2[sp][g] = m == -INFINITY ? 0.0f : expf(m - Mn);
-            }
-            __syncthreads();
-            for (int it = it0; it < items; it += FA_WARPS * 32) {
-                const int g = it / (D / 4), e4 = it % (D / 4);
-                const int row = tok * n_head + h0 + g;
-                const float4 * src = (const float4 *)(ws + (int64_t)row * (D + 4)) + e4;
-                float4 a = make_float4(0, 0, 0, 0);
-                float l = 0.0f;                                     // every thread sums its head's denominators itself (same order as the accumulators)
-#pragma unroll 1
-                for (int sp0 = 0; sp0 < n_splits; sp0 += NB) {
-                    if (sp0 > 0 || it != it0) {
-#pragma unroll
-                        for (int j = 0; j < NB; j++) if (sp0 + j < n_splits) v[j] = __ldcg(src + (int64_t)(sp0 + j) * sstride);
-                    }
-#pragma unroll
-                    for (int j = 0; j < NB; j++) {
-                        if (sp0 + j < n_splits) {
-                            const float sc = s_m2[sp0 + j][g];
-                            a.x = fmaf(v[j].x, sc, a.x); a.y = fmaf(v[j].y, sc, a.y); a.z = fmaf(v[j].z, sc, a.z); a.w = fmaf(v[j].w, sc, a.w);
-                            l += s_l[sp0 + j][g] * sc;
-                        }
-                    }
-                }
-                const float inv = 1.0f / l;
-                *(float4 *)(dst + (int64_t)row * D + e4 * 4) = make_float4(a.x * inv, a.y * inv, a.z * inv, a.w * inv);
+        for (int r = 0; r < FA_MAX_CLUSTER; r++) {
+            if (r < n_splits) {
+                pm[r] = ld_cluster_f32(cluster_map(&cM[g], r));
+                pl[r] = ld_cluster_f32(cluster_map(&cL[g], r));
+                pa[r] = ld_cluster_f32(cluster_map(&cA[g][e], r));
             }
         }
+        float Mn = -INFINITY;
+#pragma unroll
+        for (int r = 0; r < FA_MAX_CLUSTER; r++) if (r < n_splits) Mn = fmaxf(Mn, pm[r]);
+        float a = 0.0f, l = 0.0f;
+#pragma unroll
+        for (int r = 0; r < FA_MAX_CLUSTER; r++) {
+            if (r < n_splits) {
+                const float sc = pm[r] == -INFINITY ? 0.0f : expf(pm[r] - Mn);
+                a = fmaf(pa[r], sc, a);
+                l += pl[r] * sc;
+            }
+        }
+        dst[((int64_t)tok * n_head + h0 + g) * D + e] = a * (1.0f / l);            // ops.cpp:8390-8392
     }
-    if (fu.early_trigger == 0 || (fu.early_trigger == 2 && n_splits <= 1)) pdl_trigger();
+    B200_TRACE_AT(tr, 7);                     // this CTA's slice of the output written
+    // the peers' shared memory must outlive every read of it.  Relaxed: those reads have returned (their values are in dst), so no
+    // memory ordering is needed, and a release here would wait for the dst stores to drain (MEMBAR.GPU)
+    cluster_arrive_relaxed();
+    cluster_wait();
     B200_TRACE_CLOSE(tr, 10);
 }
 B200_TRACE_DUMP(b200_fa_trace_dump, g_fa_trace)
 
-// KV splits: ~2 CTAs of 128 threads per SM, at least 32 positions per split, at most FA_MAX_SPLITS
+// KV splits = the cluster size: enough CTAs for two on every SM (132 on an H100), at least 32 positions per split, at most 16 (the
+// largest cluster Hopper runs; above 8 it is a non-portable size).  Llama-3-8B decode (32 heads, 8 KV heads, G = 2) at n_kv 768:
+// 16 tiles x 16 splits of 48 positions = 256 CTAs
 static int fa_splits(int64_t n_tiles, int64_t n_tok, int64_t n_kv, int * split_len) {
-    const int sms = b200_sm_count();
-    int64_t base = n_tiles * n_tok;
-    static const int factor = getenv("B200_FA_SPLIT_FACTOR") ? atoi(getenv("B200_FA_SPLIT_FACTOR")) : 2;   // CTAs per SM aimed for
-    int64_t want = ((int64_t)factor * sms + base - 1) / base;
-    static const int minlen = getenv("B200_FA_MIN_SPLIT") ? atoi(getenv("B200_FA_MIN_SPLIT")) : 32;     // positions per split, at least
-    int64_t maxs = (n_kv + minlen - 1) / minlen;
-    if (maxs > FA_MAX_SPLITS) maxs = FA_MAX_SPLITS;
+    const int64_t base = n_tiles * n_tok;
+    int64_t want = (2 * b200_sm_count() + base - 1) / base;
+    int64_t maxs = (n_kv + 31) / 32;
+    if (maxs > FA_MAX_CLUSTER) maxs = FA_MAX_CLUSTER;
     if (want > maxs) want = maxs;
     if (want < 1) want = 1;
     int64_t len = (n_kv + want - 1) / want;
-    len = (len + minlen - 1) / minlen * minlen;
+    len = (len + 7) / 8 * 8;
     *split_len = (int)len;
     return (int)((n_kv + len - 1) / len);
 }
 
-// workspace = [FA_COUNTER_BYTES of u32 completion counters, one per (token, head tile)] [split partials
-// [splits][n_tok][n_head][dv + 4] f32].  The counter region sits at a FIXED offset so that calls with different shapes
-// never reinterpret old partials as counters; it must be zero-initialised ONCE by the caller (the counters clean
-// themselves after every launch).
-#define FA_COUNTER_BYTES (256 * 1024)
-static int64_t fa_partial_bytes(int64_t dv, int64_t n_head, int64_t n_tok, int64_t n_kv) {
-    int sl = 0;
-    int64_t maxs = fa_splits((n_head + 3) / 4, n_tok, n_kv, &sl);      // fewest head tiles (G = 4) -> most splits: an upper bound
-    return (maxs * n_tok * n_head * (dv + 4) * (int64_t)sizeof(float) + 255) & ~(int64_t)255;
-}
+// The splits merge inside their cluster: the attention needs no global workspace any more.  The entry point stays for callers
+// that size one (0 bytes; a null workspace is accepted).
 extern "C" int64_t b200_flash_attn_workspace(int64_t dv, int64_t n_head, int64_t n_tok, int64_t n_kv) {
-    return FA_COUNTER_BYTES + fa_partial_bytes(dv, n_head, n_tok, n_kv) + 256;
+    (void)dv; (void)n_head; (void)n_tok; (void)n_kv;
+    return 0;
 }
 
 template <int D, int KVT, int G>
 static int fa_launch(const float * q, int64_t q_ts, int64_t q_hs, const void * k, int64_t k_rs, int64_t k_hs,
-                     const void * v, int64_t v_rs, int64_t v_hs, const void * mask, int64_t mask_rs, float * dst, float * ws,
+                     const void * v, int64_t v_rs, int64_t v_hs, const void * mask, int64_t mask_rs, float * dst,
                      int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv, float scale, float max_bias, float softcap, cudaStream_t st, const FaFuse & fu) {
     int split_len = 0;
     const int n_tiles = (int)(n_head / G);
@@ -512,15 +485,13 @@ static int fa_launch(const float * q, int64_t q_ts, int64_t q_hs, const void * k
     const float m0 = powf(2.0f, -(max_bias) / (float)nh_log2), m1 = powf(2.0f, -(max_bias / 2.0f) / (float)nh_log2);
     if (softcap != 0.0f) scale /= softcap;
     dim3 grid((unsigned)n_splits, (unsigned)n_tiles, (unsigned)n_tok);
-    unsigned int * counters = (unsigned int *)ws;
-    if (ws) ws = (float *)((uint8_t *)ws + FA_COUNTER_BYTES);
     static const bool no_lean = getenv("B200_FA_NO_LEAN") != nullptr;
-    if (!no_lean && fu.enabled && fu.tab_mode == 1 && fu.rope_tab && mask && max_bias == 0.0f && softcap == 0.0f && n_tok == 1) {
-        B200_CUDA(b200_launch_pdl(fattn_vec_kernel<D, KVT, G, 1>, grid, dim3(FA_WARPS * 32), 0, st, q, q_ts, q_hs, (const uint8_t *)k, k_rs, k_hs, (const uint8_t *)v, v_rs, v_hs,
-            (const uint16_t *)mask, mask_rs, dst, ws, counters, (int)n_head, (int)n_head_kv, (int)n_kv, split_len, n_splits, scale, max_bias, softcap, m0, m1, nh_log2, fu));
-    } else
-    B200_CUDA(b200_launch_pdl(fattn_vec_kernel<D, KVT, G>, grid, dim3(FA_WARPS * 32), 0, st, q, q_ts, q_hs, (const uint8_t *)k, k_rs, k_hs, (const uint8_t *)v, v_rs, v_hs,
-        (const uint16_t *)mask, mask_rs, dst, ws, counters, (int)n_head, (int)n_head_kv, (int)n_kv, split_len, n_splits, scale, max_bias, softcap, m0, m1, nh_log2, fu));
+    const bool lean = !no_lean && fu.enabled && fu.tab_mode == 1 && fu.rope_tab && mask && max_bias == 0.0f && softcap == 0.0f && n_tok == 1;
+    auto kern = lean ? fattn_vec_kernel<D, KVT, G, 1> : fattn_vec_kernel<D, KVT, G, 0>;
+    if (n_splits > 8) B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    B200_CUDA(b200_launch_pdl_cluster(kern, grid, dim3(FA_WARPS * 32), 0, st, (unsigned)n_splits, q, q_ts, q_hs, (const uint8_t *)k, k_rs, k_hs,
+        (const uint8_t *)v, v_rs, v_hs, (const uint16_t *)mask, mask_rs, dst, (int)n_head, (int)n_head_kv, (int)n_kv, split_len, n_splits,
+        scale, max_bias, softcap, m0, m1, nh_log2, fu));
     b200_count_launch();
     return B200_OK;
 }
@@ -530,35 +501,33 @@ int  b200_fattn_tc(const float * q, int64_t q_ts, int64_t q_hs, const void * k, 
                    const void * mask, int64_t mask_rs, float * dst, int kv_type, int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv,
                    float scale, float softcap, void * stream);
 
-// when the attention launch lets its dependent (the wo projection) start: 0 = at the very end, 1 = at the top (measured slower: the weight burst
-// delays the K / V loads), 2 = once every CTA has written its partials, i.e. during the split merge (default)
-static int fa_early_trigger() { static const int v = getenv("B200_FA_EARLY_TRIGGER") ? atoi(getenv("B200_FA_EARLY_TRIGGER")) : 2; return v; }
 static int fa_dispatch(const float * q, int64_t q_ts, int64_t q_hs, const void * k, int64_t k_rs, int64_t k_hs,
                                    const void * v, int64_t v_rs, int64_t v_hs, const void * mask, int64_t mask_rs, float * dst,
                                    int kv_type, int64_t dk, int64_t dv, int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv,
-                                   float scale, float max_bias, float softcap, void * workspace, void * stream, const FaFuse & fu) {
+                                   float scale, float max_bias, float softcap, void * stream, const FaFuse & fu) {
     if (!q || !k || !v || !dst) { b200_set_error("flash_attn: null pointer"); return B200_ERR_INVALID; }
     if (dk != dv || (dk != 64 && dk != 128)) { b200_set_error("flash_attn: head size %lld/%lld unsupported (64 or 128)", (long long)dk, (long long)dv); return B200_ERR_UNSUPPORTED; }
     if (kv_type != B200_TYPE_F16 && kv_type != B200_TYPE_Q8_0) { b200_set_error("flash_attn: kv type %d unsupported", kv_type); return B200_ERR_UNSUPPORTED; }
     if (n_head_kv <= 0 || n_head % n_head_kv != 0 || n_tok <= 0 || n_kv <= 0) { b200_set_error("flash_attn: bad head counts"); return B200_ERR_INVALID; }
     if (((uintptr_t)q & 15) || (q_ts & 3) || (q_hs & 3)) { b200_set_error("flash_attn: q must be 16-byte aligned"); return B200_ERR_INVALID; }
     if (kv_type == B200_TYPE_F16 && ((((uintptr_t)k | (uintptr_t)v) & 15) || ((k_rs | k_hs | v_rs | v_hs) & 15))) { b200_set_error("flash_attn: f16 K/V rows must be 16-byte aligned"); return B200_ERR_INVALID; }
-    if (n_tok > 65535 || n_tok * n_head * (int64_t)sizeof(unsigned int) > FA_COUNTER_BYTES) { b200_set_error("flash_attn: n_tok * n_head too large for one launch"); return B200_ERR_UNSUPPORTED; }
+    if (n_tok > 65535) { b200_set_error("flash_attn: n_tok * n_head too large for one launch"); return B200_ERR_UNSUPPORTED; }
     // multi-token batches (prefill, big verify batches): the tensor-core kernel (fattn_tc.cu) — K / V read once per 128 query tokens
     if (!fu.enabled && b200_fattn_tc_supported(kv_type, dk, dv, n_tok, n_kv, max_bias) && (!mask || ((mask_rs & 7) == 0 && ((uintptr_t)mask & 15) == 0)) &&
         (kv_type != B200_TYPE_F16 || (((k_rs | k_hs | v_rs | v_hs) & 15) == 0)))
         return b200_fattn_tc(q, q_ts, q_hs, k, k_rs, k_hs, v, v_rs, v_hs, mask, mask_rs, dst, kv_type, n_head, n_head_kv, n_tok, n_kv, scale, softcap, stream);
     const int64_t gq = n_head / n_head_kv;
-    const int G = gq % 4 == 0 ? 4 : (gq % 2 == 0 ? 2 : 1);
-    if (!workspace && (n_kv + 31) / 32 > 1) { b200_set_error("flash_attn: workspace required"); return B200_ERR_INVALID; }
-    cudaStream_t st = (cudaStream_t)stream; float * ws = (float *)workspace;
-#define FA_CASE(DD, KK, GG) return fa_launch<DD, KK, GG>(q, q_ts, q_hs, k, k_rs, k_hs, v, v_rs, v_hs, mask, mask_rs, dst, ws, n_head, n_head_kv, n_tok, n_kv, scale, max_bias, softcap, st, fu)
+    // query heads per CTA.  G = 4 halves the K/V reads from L2 but leaves half as many CTAs to keep loads in flight: on an H100 SXM
+    // (400 W) Llama-3-8B decode ran 407 tok/s with G = 4 (8 tiles x 16 splits, one CTA per SM) and 415 tok/s with G = 2 (16 x 16)
+    const int G = gq % 2 == 0 ? 2 : 1;
+    cudaStream_t st = (cudaStream_t)stream;
+#define FA_CASE(DD, KK, GG) return fa_launch<DD, KK, GG>(q, q_ts, q_hs, k, k_rs, k_hs, v, v_rs, v_hs, mask, mask_rs, dst, n_head, n_head_kv, n_tok, n_kv, scale, max_bias, softcap, st, fu)
     if (dk == 128) {
-        if (kv_type == B200_TYPE_F16) { if (G == 4) FA_CASE(128, B200_TYPE_F16, 4); if (G == 2) FA_CASE(128, B200_TYPE_F16, 2); FA_CASE(128, B200_TYPE_F16, 1); }
-        else                          { if (G == 4) FA_CASE(128, B200_TYPE_Q8_0, 4); if (G == 2) FA_CASE(128, B200_TYPE_Q8_0, 2); FA_CASE(128, B200_TYPE_Q8_0, 1); }
+        if (kv_type == B200_TYPE_F16) { if (G == 2) FA_CASE(128, B200_TYPE_F16, 2); FA_CASE(128, B200_TYPE_F16, 1); }
+        else                          { if (G == 2) FA_CASE(128, B200_TYPE_Q8_0, 2); FA_CASE(128, B200_TYPE_Q8_0, 1); }
     } else {
-        if (kv_type == B200_TYPE_F16) { if (G == 4) FA_CASE(64, B200_TYPE_F16, 4); if (G == 2) FA_CASE(64, B200_TYPE_F16, 2); FA_CASE(64, B200_TYPE_F16, 1); }
-        else                          { if (G == 4) FA_CASE(64, B200_TYPE_Q8_0, 4); if (G == 2) FA_CASE(64, B200_TYPE_Q8_0, 2); FA_CASE(64, B200_TYPE_Q8_0, 1); }
+        if (kv_type == B200_TYPE_F16) { if (G == 2) FA_CASE(64, B200_TYPE_F16, 2); FA_CASE(64, B200_TYPE_F16, 1); }
+        else                          { if (G == 2) FA_CASE(64, B200_TYPE_Q8_0, 2); FA_CASE(64, B200_TYPE_Q8_0, 1); }
     }
 #undef FA_CASE
     return B200_ERR_UNSUPPORTED;
@@ -568,9 +537,9 @@ extern "C" int b200_flash_attn_ext(const float * q, int64_t q_ts, int64_t q_hs, 
                                    const void * v, int64_t v_rs, int64_t v_hs, const void * mask, int64_t mask_rs, float * dst,
                                    int kv_type, int64_t dk, int64_t dv, int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv,
                                    float scale, float max_bias, float softcap, void * workspace, void * stream) {
+    (void)workspace;                          // no longer needed: the splits merge inside their cluster
     FaFuse fu; memset(&fu, 0, sizeof(fu));
-    fu.early_trigger = fa_early_trigger();
-    return fa_dispatch(q, q_ts, q_hs, k, k_rs, k_hs, v, v_rs, v_hs, mask, mask_rs, dst, kv_type, dk, dv, n_head, n_head_kv, n_tok, n_kv, scale, max_bias, softcap, workspace, stream, fu);
+    return fa_dispatch(q, q_ts, q_hs, k, k_rs, k_hs, v, v_rs, v_hs, mask, mask_rs, dst, kv_type, dk, dv, n_head, n_head_kv, n_tok, n_kv, scale, max_bias, softcap, stream, fu);
 }
 
 extern "C" int b200_rope_kv_flash_attn2(const float * q_src, float * q_dst, const float * k_new, const float * v_new, const int32_t * pos, const float * ff,
@@ -599,10 +568,11 @@ extern "C" int b200_rope_kv_flash_attn2(const float * q_src, float * q_dst, cons
     const int64_t hs = kv_type == B200_TYPE_F16 ? hd * 2 : hd / 32 * 34;
     if (k_hs != hs || v_hs != hs) { b200_set_error("rope_kv_flash_attn: heads must be contiguous inside a cache cell"); return B200_ERR_INVALID; }
     if (((uintptr_t)q_src | (uintptr_t)q_dst | (uintptr_t)k_new | (uintptr_t)v_new | (uintptr_t)rope_tab) & 15) { b200_set_error("rope_kv_flash_attn: 16-byte alignment required"); return B200_ERR_INVALID; }
+    (void)workspace;
     FaFuse fu; memset(&fu, 0, sizeof(fu));
     fu.q_src = q_src; fu.q_dst = q_dst; fu.k_new = k_new; fu.v_new = v_new; fu.pos = pos; fu.ff = ff; fu.k_ids = k_ids; fu.v_ids = v_ids;
-    fu.rp = rope_host_params(p); fu.enabled = 1; fu.early_trigger = fa_early_trigger(); fu.trace = b200_trace_on() ? 1 : 0;
+    fu.rp = rope_host_params(p); fu.enabled = 1; fu.trace = b200_trace_on() ? 1 : 0;
     fu.rope_tab = rope_tab; fu.tab_mode = rope_tab ? tab_mode : 0;
     return fa_dispatch(q_dst, hd * n_head, hd, k_cache, k_rs, k_hs, v_cache, v_rs, v_hs, mask, 0, dst, kv_type, hd, hd, n_head, n_head_kv, 1, n_kv,
-                       scale, max_bias, softcap, workspace, stream, fu);
+                       scale, max_bias, softcap, stream, fu);
 }

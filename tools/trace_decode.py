@@ -48,7 +48,7 @@ def main():
         cta = r[8] >> 48; pairs = (r[8] >> 16) & 0xffffffff; typ = (r[8] >> 8) & 0xff; nm = r[8] & 0xff
         recs.append(("mmvq", r, f"cta {cta:3d} units {pairs:6d} type {typ:2d} mats {nm} k {r[9]}"))
     for r in fa:
-        recs.append(("attn", r, f"split {r[8] >> 48:2d}/{r[8] & 0xffff} n_kv {(r[8] >> 16) & 0xffffffff}{' MERGER' if r[9] else ''}"))
+        recs.append(("attn", r, f"split {r[8] >> 48:2d}/{r[8] & 0xffff} n_kv {(r[8] >> 16) & 0xffffffff}"))
     recs.sort(key=lambda x: x[1][0])
     t0 = recs[0][1][0]
     # SM clock per ns from the longest record
@@ -56,11 +56,11 @@ def main():
     ghz = (best[10] - best[1]) / max(1, best[11] - best[0])
     print(f"# SM clock ~{ghz:.3f} GHz (clock64 / globaltimer over the longest record); times in us; columns = deltas between consecutive stamps")
     print("# mmvq: entry->primed | ->prev kernel done (griddepcontrol.wait) | ->activations ready | ->warp0 first slot | ->warp0 done | ->CTA done")
-    print("# attn: entry->K/V requested | ->QKV done (wait) | ->rope+stage | ->positions done | ->partials+count | ->exit (merge if MERGER)")
+    print("# attn: entry->K/V requested | ->QKV done (wait) | ->rope+stage | ->positions done | ->cluster's partials published | ->slice merged | ->exit")
     last_end = None
     for kind, r, info in recs:
-        c = [r[1], r[2], r[3], r[4], r[5], r[6], r[10]]
-        d = [(c[i + 1] - c[i]) / ghz / 1e3 if c[i + 1] and c[i] else float("nan") for i in range(6)]
+        c = [r[1], r[2], r[3], r[4], r[5], r[6]] + ([r[7]] if kind == "attn" else []) + [r[10]]
+        d = [(c[i + 1] - c[i]) / ghz / 1e3 if c[i + 1] and c[i] else float("nan") for i in range(len(c) - 1)]
         start = (r[0] - t0) / 1e3; end = (r[11] - t0) / 1e3
         gap = "" if last_end is None else f" (start {start - last_end:+6.2f} vs prev end)"
         print(f"{start:9.2f} {kind} dur {end - start:6.2f} | " + " ".join(f"{x:6.2f}" for x in d) + f" | {info}{gap}")
