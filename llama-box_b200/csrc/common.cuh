@@ -156,6 +156,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t * bar, uint32_t parity) {
         "DONE_%=:\n\t}"
         :: "r"(smem_u32(bar)), "r"(parity) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t * bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
+}
+// wait on an mbarrier, optionally accounting the cycles to a profile counter
+__device__ __forceinline__ void mbar_wait_p(uint64_t * bar, uint32_t parity, unsigned long long * acc) {
+    if (acc) { const long long t0 = clock64(); mbar_wait(bar, parity); *acc += (unsigned long long)(clock64() - t0); }
+    else mbar_wait(bar, parity);
+}
+// generic-proxy shared-memory writes -> visible to the async proxy (tensor core operands, bulk copies)
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // global -> shared bulk copy; src/dst 16-byte aligned, bytes % 16 == 0; completes on `bar`
 __device__ __forceinline__ void bulk_g2s(void * smem_dst, const void * gsrc, uint32_t bytes, uint64_t * bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"

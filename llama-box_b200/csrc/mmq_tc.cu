@@ -115,11 +115,6 @@ __global__ void __launch_bounds__(256) quantize_mmq_kernel(const float * __restr
     pdl_trigger();
 }
 
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint64_t * bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-
 struct TcArgs {
     const uint8_t * W;          // weights, `type` rows (Q6_K: repacked rows, see repack.cu)
     const uint8_t * ws;         // B image (quantize_mmq_kernel)
@@ -130,12 +125,6 @@ struct TcArgs {
     uint32_t lbo, sbo;          // descriptor strides (bytes): K-chunk stride / 8-row-group stride
     unsigned long long * prof;  // bring-up: per-role cycle counters of CTA 0 (B200_MMQ_PROF), normally null
 };
-// wait on an mbarrier, optionally accounting the cycles to a profile counter
-__device__ __forceinline__ void mbar_wait_p(uint64_t * bar, uint32_t parity, unsigned long long * acc) {
-    if (acc) { const long long t0 = clock64(); mbar_wait(bar, parity); *acc += (unsigned long long)(clock64() - t0); }
-    else mbar_wait(bar, parity);
-}
-
 // ---- per-type pipeline geometry: K-stages per super-block, whether the mins MMA runs, activation bytes per stage -------
 // (the transform threads read each row's packed blocks straight from global memory, so no weight bytes live in shared memory;
 // Q6_K rows are repacked [ql 128B x nb][qh 64B x nb][scales 16B x nb][d f16 x nb], see repack.cu)
@@ -435,6 +424,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
+unsigned long long * b200_mmq_prof_buf();
+void b200_mmq_prof_report(const char * kernel, int type, int64_t m, int64_t k, int64_t ncols, int n_tiles, cudaStream_t st);
+
 bool b200_mmq_tc_supported(int type, int64_t m, int64_t k, int64_t ncols) {
     static const bool off = getenv("B200_MMQ_DISABLE_TC") != nullptr;     // debugging: stream column groups through the matvec kernel instead (still the GPU)
     if (off || m <= 0 || ncols < 9) return false;
@@ -462,10 +454,7 @@ int b200_mmq_tc(int type, const void * W, const float * X, int64_t x_col_stride,
     a.rb = (k / 256) * type_block_bytes(type);
     a.g = tc_geom(k, ncols);
     a.lbo = (uint32_t)TC_PANEL; a.sbo = 128u;
-    static unsigned long long * prof_buf = nullptr;                        // B200_MMQ_PROF=1: per-role wait cycles of CTA 0, printed after each launch (bring-up only)
-    static const bool want_prof = getenv("B200_MMQ_PROF") != nullptr;
-    if (want_prof && !prof_buf) { cudaMalloc((void **)&prof_buf, 16 * 4 * 8); }
-    a.prof = want_prof ? prof_buf : nullptr;
+    a.prof = b200_mmq_prof_buf();
     a.nsb = (int32_t)(k / 256); a.n_mtiles = (int32_t)((m + TC_TM - 1) / TC_TM); a.n_tiles = (int32_t)(a.n_mtiles * a.g.nt); a.type = type;
     dim3 qgrid((unsigned)a.nsb, (unsigned)(a.g.nt * 16));
     B200_CUDA(b200_launch_pdl(quantize_mmq_kernel, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k, (uint8_t *)workspace, a.g));
@@ -476,14 +465,24 @@ int b200_mmq_tc(int type, const void * W, const float * X, int64_t x_col_stride,
         case B200_TYPE_Q5_K: rc = tc_launch<B200_TYPE_Q5_K>(a, st); break;
         case B200_TYPE_Q6_K: rc = tc_launch<B200_TYPE_Q6_K>(a, st); break;
     }
-    if (want_prof && rc == B200_OK) {
-        unsigned long long h[16 * 4];
-        cudaStreamSynchronize(st); cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
-        const char * role[12] = { "mma", "mma", "mma", "mma", "mma", "mma", "mma", "mma", "xform", "xform", "xform", "xform" };
-        fprintf(stderr, "mmq_tc prof (CTA 0, cycles): type %d m %lld k %lld n %lld tiles %d\n", type, (long long)m, (long long)k, (long long)ncols, a.n_tiles);
-        for (int w = 0; w < 12; w += (w < 8 ? 4 : 2))
-            fprintf(stderr, "  warp %2d %-8s total %9llu  wait0 %9llu  wait1 %9llu  wait2 %9llu\n", w, role[w], h[w * 4], h[w * 4 + 1], h[w * 4 + 2], h[w * 4 + 3]);
-        fprintf(stderr, "  (mma: wait0 = b_full, wait1 = a_full | xform: wait1 = ab_empty)\n");
-    }
+    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc", type, m, k, ncols, a.n_tiles, st);
     return rc;
+}
+
+// B200_MMQ_PROF=1: per-role wait cycles of CTA 0 of the tile kernels (this file and mmq_tc32.cu, which share the warp roles),
+// printed after each launch (bring-up only)
+unsigned long long * b200_mmq_prof_buf() {
+    static unsigned long long * prof_buf = nullptr;
+    static const bool want_prof = getenv("B200_MMQ_PROF") != nullptr;
+    if (want_prof && !prof_buf) { cudaMalloc((void **)&prof_buf, 16 * 4 * 8); }
+    return want_prof ? prof_buf : nullptr;
+}
+void b200_mmq_prof_report(const char * kernel, int type, int64_t m, int64_t k, int64_t ncols, int n_tiles, cudaStream_t st) {
+    unsigned long long h[16 * 4];
+    cudaStreamSynchronize(st); cudaMemcpy(h, b200_mmq_prof_buf(), sizeof(h), cudaMemcpyDeviceToHost);
+    const char * role[12] = { "mma", "mma", "mma", "mma", "mma", "mma", "mma", "mma", "xform", "xform", "xform", "xform" };
+    fprintf(stderr, "%s prof (CTA 0, cycles): type %d m %lld k %lld n %lld tiles %d\n", kernel, type, (long long)m, (long long)k, (long long)ncols, n_tiles);
+    for (int w = 0; w < 12; w += (w < 8 ? 4 : 2))
+        fprintf(stderr, "  warp %2d %-8s total %9llu  wait0 %9llu  wait1 %9llu  wait2 %9llu\n", w, role[w], h[w * 4], h[w * 4 + 1], h[w * 4 + 2], h[w * 4 + 3]);
+    fprintf(stderr, "  (mma: wait0 = b_full, wait1 = a_full | xform: wait1 = ab_empty)\n");
 }

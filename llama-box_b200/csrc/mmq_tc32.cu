@@ -1,0 +1,333 @@
+// mmq_tc32.cu — batched MUL_MAT on Q4_0 / Q5_0 / Q8_0 weights (prefill / large ubatches) on the Hopper tensor cores (sm_90a):
+// int8 wgmma (SASS: IGMMA) with s32 register accumulators, TMA (cp.async.bulk) staging, warp-specialised, persistent.
+// The sibling of mmq_tc.cu (K-quants) for the formats whose scale is an f16 per 32 elements on BOTH operands.
+//
+// The arithmetic is the CPU ORACLE's (oracle.c dot_q4_0 / dot_q5_0 / dot_q8_0), as in the matvec (mmvq.cu): activations are
+// quantised to q8_0 exactly like b200_quantize_act2(kind 1) (d = max / 127 -> f16, id = 127 / max, RNE), the integer sum of each
+// 32-element block is exact, and each block is folded into an f32 running sum with the oracle's products and roundings:
+//
+//     Q4_0:          acc += ((float)s * d_w) * d_x          Q5_0 / Q8_0:   acc += (float)s * (d_w * d_x)
+//
+// Every output has one running sum and its blocks are added in the oracle's order (block 0 first), so the result does not depend
+// on the tile schedule; the matvec (column groups) splits a row over lanes and differs from this in the f32 summation order only.
+//
+// Why int8 wgmma and not the f16-integer trick of mmq_tc.cu: with a scale per 32 elements on both sides nothing can be folded
+// into an operand, so the accumulator has to be read out after EVERY block.  One m64nNk32.s32.s8.s8 instruction is exactly one
+// block and its s32 result is exact by construction; the f16 route needs two k16 instructions and twice the shared-memory bytes
+// for the same block.  For Q8_0 the repacked row's qs run already is the A operand (the transform only places it); Q4_0 / Q5_0
+// expand nibbles (+ the qh bit) to int8 with the -8 / -16 offset applied, in natural element order (low nibbles = elements
+// 0..15 = the first 16-byte K-chunk of the block, high nibbles = the second), so the activation image needs no permutation.
+//
+// What limits it: the fold, not the tensor pipe.  Per block a consumer thread converts and scales 64 accumulators (convert, two
+// multiplies, add = 4 issue slots each) against 64 cycles of IGMMA per warpgroup, so the issue slots of the two consumer
+// warpgroups bound the kernel well below the int8 rate (counted: about a quarter; measured: a tenth, H100.md).  To keep the tensor pipe and the fold overlapped each
+// warpgroup splits its 128 columns in two m64n64k32 halves with an accumulator set each: while one half is folded the other
+// half's (or the next block's) MMA runs.  Registers: 64 f32 sums + 2 x 32 s32 accumulators, no setmaxnreg needed.
+//
+// Warp roles (384 threads, one persistent CTA per SM), as in mmq_tc.cu:
+//     warps 0-3 / 4-7  consumers: tile rows 0-63 / 64-127, all 128 columns
+//     warps 8-11       transform: thread t owns weight row t of the tile, reads its packed blocks one stage ahead from global
+//                      memory into registers; thread 0 also issues the activation panel of each stage (cp.async.bulk)
+// A stage is 128 k (4 blocks): A 16 KB (int8 core matrices) + B 16 KB + d_x 2 KB + d_w 2 KB; 4 stages, ~144 KB of shared memory.
+#include "common.cuh"
+#include "wgmma.cuh"
+
+#include <cstdlib>
+
+#define T32_TM 128
+#define T32_TN 128
+#define T32_THREADS 384
+#define T32_KS 128                  // k per stage
+#define T32_NSTAGE 4
+#define T32_PANEL 2048              // one K-chunk (16 int8 = 16 bytes) of 128 rows
+#define T32_STAGE_A (8 * T32_PANEL)
+#define T32_STAGE_B (8 * T32_PANEL + 4 * 512)      // the panel + d_x of its 4 blocks
+
+// B200_MMQ_PROF (mmq_tc.cu)
+unsigned long long * b200_mmq_prof_buf();
+void b200_mmq_prof_report(const char * kernel, int type, int64_t m, int64_t k, int64_t ncols, int n_tiles, cudaStream_t st);
+
+// ---- workspace geometry (the activation image) --------------------------------------------------------------------------
+// per 128-token tile nt and 128-k stage ks, contiguous so that one stage is one run of bytes:
+//     Q[nt][ks][chunk 0..7][n 0..127][16 int8]      element e of block b of the stage: chunk 2 b + e / 16, byte e % 16
+//     D[nt][ks][block 0..3][n 0..127] f32           d_x
+struct Tc32Geom { int64_t nt, ns, total; };
+static Tc32Geom tc32_geom(int64_t k, int64_t ncols) {
+    Tc32Geom g;
+    g.nt = (ncols + T32_TN - 1) / T32_TN; g.ns = k / T32_KS;
+    g.total = g.nt * g.ns * T32_STAGE_B;
+    return g;
+}
+
+// ---- activation quantisation into the image ------------------------------------------------------------------------------
+// one warp per (token, 256 elements), 4 lanes per q8_0 block: the arithmetic of warp_quant_q80 (actquant.cuh).  Elements from
+// k_valid up (padded weight rows) and tokens from ncols up are zeros with d = 0.
+__global__ void __launch_bounds__(256) quantize_mmq32_kernel(const float * __restrict__ x, int64_t x_col_stride, int64_t ncols, int64_t k_valid,
+                                                            uint8_t * __restrict__ ws, Tc32Geom g) {
+    pdl_wait();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t blk = blockIdx.x;
+    const int64_t n = (int64_t)blockIdx.y * 8 + warp;                // token (padded range: < nt * 128)
+    const int64_t nt = n >> 7; const int nl = (int)(n & 127);
+    float v[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
+    if (n < ncols && blk * 256 + lane * 8 < k_valid) {
+        const float4 * p = (const float4 *)(x + n * x_col_stride + blk * 256 + lane * 8);
+        const float4 a = p[0], b = p[1];
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+    }
+    float am = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 8; j++) am = fmaxf(am, fabsf(v[j]));
+    am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, 1));
+    am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, 2));
+    const float d  = __fdiv_rn(am, 127.0f);
+    const float id = am != 0.0f ? __fdiv_rn(127.0f, am) : 0.0f;
+    int q[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) q[j] = __float2int_rn(__fmul_rn(v[j], id));
+    uint2 pk;
+    pk.x = (q[0] & 0xff) | ((q[1] & 0xff) << 8) | ((q[2] & 0xff) << 16) | ((q[3] & 0xff) << 24);
+    pk.y = (q[4] & 0xff) | ((q[5] & 0xff) << 8) | ((q[6] & 0xff) << 16) | ((q[7] & 0xff) << 24);
+    uint8_t * stage = ws + ((nt * g.ns + blk * 2 + (lane >> 4)) * T32_STAGE_B);
+    const int b = (lane >> 2) & 3;                                   // block of the stage
+    *(uint2 *)(stage + (2 * b + ((lane & 3) >> 1)) * T32_PANEL + nl * 16 + (lane & 1) * 8) = pk;
+    if ((lane & 3) == 0) *(float *)(stage + 8 * T32_PANEL + (b * 128 + nl) * 4) = __half2float(__float2half_rn(d));   // the oracle stores d as f16
+    pdl_trigger();
+}
+
+struct Tc32Args {
+    const uint8_t * W;          // weights: repacked rows (repack_layout.cuh), k a multiple of 256 (padded rows included)
+    const uint8_t * ws;         // activation image (quantize_mmq32_kernel)
+    float *         dst;        // [ncols][ldd] f32
+    int64_t m, k, ncols, ldd, rb, nt;
+    int32_t ns, n_tiles;
+    unsigned long long * prof;  // per-role cycle counters of CTA 0 (B200_MMQ_PROF), normally null
+};
+
+struct Tc32Smem {
+    static constexpr int A = 0, B = A + T32_NSTAGE * T32_STAGE_A;
+    static constexpr int RS = B + T32_NSTAGE * T32_STAGE_B;          // d_w ring: stage x block x 128 rows f32
+    static constexpr int BAR = RS + T32_NSTAGE * 2048;
+    static constexpr int TOTAL = BAR + 128;
+};
+
+__device__ __forceinline__ uint32_t bit4_of(uint32_t b) { return (((b & 0xFu) * 0x00204081u) & 0x01010101u) << 4; }   // 4 bits -> bit 4 of 4 bytes
+// bytes v in [0, 2 OFF) -> v - OFF as int8, four at a time (no borrow crosses a byte: 0x80 + v - OFF >= 0x70)
+template <uint32_t OFF> __device__ __forceinline__ uint32_t recentre(uint32_t v) { return ((v | 0x80808080u) - OFF * 0x01010101u) ^ 0x80808080u; }
+
+template <int T>
+__global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_constant__ Tc32Args args) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint64_t * b_full = (uint64_t *)(smem + Tc32Smem::BAR), * a_full = b_full + T32_NSTAGE, * ab_empty = a_full + T32_NSTAGE;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+    if (tid == 0) {
+        for (int i = 0; i < T32_NSTAGE; i++) { mbar_init(&b_full[i], 1); mbar_init(&a_full[i], 4); mbar_init(&ab_empty[i], 8); }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    pdl_wait();
+
+    const int ns = args.ns;
+    const int64_t NT = args.nt;
+    unsigned long long w0 = 0, w1 = 0;                               // profile: cycles in this role's kinds of waits
+    const bool prof = args.prof != nullptr && blockIdx.x == 0;
+    unsigned long long * pw0 = prof ? &w0 : nullptr, * pw1 = prof ? &w1 : nullptr;
+    const long long t_start = clock64();
+
+    if (warp >= 8) {
+        // ===================== transform: packed blocks -> int8 core matrices + d_w =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 88;");
+        constexpr int NQ = T == B200_TYPE_Q8_0 ? 8 : 4;                  // 16-byte words of qs per row and stage
+        constexpr int QB = T == B200_TYPE_Q8_0 ? 32 : 16;                // qs bytes per block
+        const int t = tid - 8 * 32;                                      // weight row of the tile
+        const int64_t nb = args.k / 32;
+        uint32_t it = 0;
+        uint4 nxt[NQ], nxt_h = make_uint4(0, 0, 0, 0); uint2 nxt_d;
+        auto fetch = [&](int tile, int s) {
+            int64_t r = (int64_t)(tile / NT) * T32_TM + t; if (r >= args.m) r = args.m - 1;   // rows past the end: any valid row (never stored)
+            const uint8_t * row = args.W + r * args.rb;
+            const uint4 * p = (const uint4 *)(row + (int64_t)s * 4 * QB);
+#pragma unroll
+            for (int i = 0; i < NQ; i++) nxt[i] = __ldg(p + i);
+            if (T == B200_TYPE_Q5_0) nxt_h = __ldg((const uint4 *)(row + nb * 16 + (int64_t)s * 16));
+            nxt_d = __ldg((const uint2 *)(row + nb * (T == B200_TYPE_Q5_0 ? 20 : QB) + (int64_t)s * 8));
+        };
+        if (blockIdx.x < args.n_tiles) fetch(blockIdx.x, 0);
+        for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
+            for (int s = 0; s < ns; s++, it++) {
+                uint4 cur[NQ]; const uint4 cur_h = nxt_h; const uint2 cur_d = nxt_d;
+#pragma unroll
+                for (int i = 0; i < NQ; i++) cur[i] = nxt[i];
+                {   // prefetch the next stage (of this tile, or the first one of this CTA's next tile)
+                    int ntile = tile, nsi = s + 1;
+                    if (nsi == ns) { nsi = 0; ntile = tile + gridDim.x; }
+                    if (ntile < args.n_tiles) fetch(ntile, nsi);
+                }
+                const int st = it % T32_NSTAGE;
+                mbar_wait_p(&ab_empty[st], ((it / T32_NSTAGE) & 1) ^ 1, pw1);
+                if (t == 0) {
+                    mbar_expect_tx(&b_full[st], (uint32_t)T32_STAGE_B);
+                    const uint8_t * src = args.ws + (((int64_t)(tile % NT) * ns + s) * T32_STAGE_B);
+                    for (int o = 0; o < T32_STAGE_B; o += T32_STAGE_B / 3) bulk_g2s(smem + Tc32Smem::B + st * T32_STAGE_B + o, src + o, T32_STAGE_B / 3, &b_full[st]);
+                }
+                uint8_t * As = smem + Tc32Smem::A + st * T32_STAGE_A + t * 16;
+                if (T == B200_TYPE_Q8_0) {
+#pragma unroll
+                    for (int c = 0; c < 8; c++) *(uint4 *)(As + c * T32_PANEL) = cur[c];
+                } else {
+                    const uint32_t qh[4] = { cur_h.x, cur_h.y, cur_h.z, cur_h.w };
+#pragma unroll
+                    for (int b = 0; b < 4; b++) {
+                        const uint32_t w[4] = { cur[b].x, cur[b].y, cur[b].z, cur[b].w };
+                        uint4 lo, hi;
+                        uint32_t * plo = (uint32_t *)&lo, * phi = (uint32_t *)&hi;
+#pragma unroll
+                        for (int i = 0; i < 4; i++) {
+                            const uint32_t l = w[i] & 0x0F0F0F0Fu, h = (w[i] >> 4) & 0x0F0F0F0Fu;
+                            if (T == B200_TYPE_Q4_0) { plo[i] = recentre<8>(l); phi[i] = recentre<8>(h); }
+                            else { plo[i] = recentre<16>(l | bit4_of(qh[b] >> (4 * i))); phi[i] = recentre<16>(h | bit4_of(qh[b] >> (16 + 4 * i))); }   // qh bit j -> element j
+                        }
+                        *(uint4 *)(As + (2 * b) * T32_PANEL) = lo;              // elements 0..15: low nibbles
+                        *(uint4 *)(As + (2 * b + 1) * T32_PANEL) = hi;          // elements 16..31: high nibbles
+                    }
+                }
+                float * rs = (float *)(smem + Tc32Smem::RS + st * 2048) + t;
+                rs[0]   = h2f((uint16_t)(cur_d.x & 0xffff)); rs[128] = h2f((uint16_t)(cur_d.x >> 16));
+                rs[256] = h2f((uint16_t)(cur_d.y & 0xffff)); rs[384] = h2f((uint16_t)(cur_d.y >> 16));
+                fence_async_smem();                                       // generic-proxy writes -> visible to the tensor core (async proxy)
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&a_full[st]);
+            }
+        }
+    } else {
+        // ===================== consumers: one IGMMA per (block, column half), fold into f32 running sums, store =====================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");           // 2 x 128 x 208 + 128 x 88 = the 384 x 168 the CTA was launched with
+        const int g = warp >> 2;
+        const int ra = 64 * g + 16 * (warp & 3) + (lane >> 2);          // tile rows ra, ra + 8 (wgmma accumulator layout, wgmma.cuh)
+        const int c0 = 2 * (lane & 3);                                  // tile columns 8 j + c0 + {0, 1}
+        uint32_t it = 0;
+        for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
+            const int64_t mt = tile / NT, nt = tile % NT;
+            float acc[64];
+            int32_t f0[32], f1[32];                                      // accumulators of column halves 0-63 / 64-127
+#pragma unroll
+            for (int c = 0; c < 64; c++) acc[c] = 0.0f;
+#pragma unroll
+            for (int c = 0; c < 32; c++) { f0[c] = 0; f1[c] = 0; }
+            auto mma = [&](int32_t (&f)[32], int st, int b, int h) {
+                const uint32_t a = smem_u32(smem + Tc32Smem::A + st * T32_STAGE_A) + g * 1024 + b * 2 * T32_PANEL;
+                const uint32_t bb = smem_u32(smem + Tc32Smem::B + st * T32_STAGE_B) + h * 1024 + b * 2 * T32_PANEL;
+                wg_fence();
+                wg_mma_ss_s8(f, wg_desc(a, T32_PANEL, 128u), wg_desc(bb, T32_PANEL, 128u), 0u);
+                wg_commit();
+            };
+            auto fold = [&](int32_t (&f)[32], int st, int b, int h) {
+                const float * rs = (const float *)(smem + Tc32Smem::RS + st * 2048) + b * 128;
+                const float da = rs[ra], db = rs[ra + 8];
+                const float2 * dx2 = (const float2 *)(smem + Tc32Smem::B + st * T32_STAGE_B + 8 * T32_PANEL + (b * 128 + 64 * h + c0) * 4);
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    const float2 dxp = dx2[4 * j];
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const float dx = e ? dxp.y : dxp.x;
+                        float & ua = acc[4 * (8 * h + j) + e], & ub = acc[4 * (8 * h + j) + 2 + e];
+                        const float sa = (float)f[4 * j + e], sb = (float)f[4 * j + 2 + e];
+                        if (T == B200_TYPE_Q4_0) {                                  // ((float)s * d_w) * d_x
+                            ua = __fadd_rn(ua, __fmul_rn(__fmul_rn(sa, da), dx));
+                            ub = __fadd_rn(ub, __fmul_rn(__fmul_rn(sb, db), dx));
+                        } else {                                                    // (float)s * (d_w * d_x)
+                            ua = __fadd_rn(ua, __fmul_rn(sa, __fmul_rn(da, dx)));
+                            ub = __fadd_rn(ub, __fmul_rn(sb, __fmul_rn(db, dx)));
+                        }
+                    }
+                }
+            };
+            for (int s = 0; s < ns; s++, it++) {
+                const int st = it % T32_NSTAGE;
+                mbar_wait_p(&b_full[st], (it / T32_NSTAGE) & 1, pw0);
+                mbar_wait_p(&a_full[st], (it / T32_NSTAGE) & 1, pw1);
+                // straight-line software pipeline over the 4 blocks of the stage: one half's MMA runs while the other half is folded
+                mma(f0, st, 0, 0);
+#pragma unroll
+                for (int b = 0; b < 4; b++) {
+                    mma(f1, st, b, 1);
+                    wg_wait1(); wg_pin(f0);
+                    fold(f0, st, b, 0);
+                    if (b < 3) { mma(f0, st, b + 1, 0); wg_wait1(); } else wg_wait0();
+                    wg_pin(f1);
+                    fold(f1, st, b, 1);
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&ab_empty[st]);                // every MMA and every scale read of the stage is done
+            }
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int64_t row = mt * T32_TM + ra + 8 * h;
+                if (row >= args.m) continue;
+#pragma unroll
+                for (int j = 0; j < 16; j++) {
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int64_t n = nt * T32_TN + 8 * j + c0 + e;
+                        if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
+                    }
+                }
+            }
+        }
+    }
+
+    if (prof && lane == 0) {                                           // [warp][total, wait0, wait1, wait2]
+        unsigned long long * o = args.prof + warp * 4;
+        o[0] = (unsigned long long)(clock64() - t_start); o[1] = w0; o[2] = w1; o[3] = 0;
+    }
+    pdl_trigger();
+}
+
+// ---- host ----------------------------------------------------------------------------------------------------------
+// Fewest activation columns that go to the tensor cores; below it the columns stream through the matvec in groups of 8.  A tile pass
+// costs the same for 9 columns as for 128 (and a matrix of m rows occupies only m / 128 SMs), a column group costs one pass over the
+// weights.  Measured on the Llama-3-8B shapes at Q8_0 (H100.md): at 32 columns the column groups win on three shapes of four, at 64
+// the tensor cores win on all four; by the per-group time in between, 7 groups (49 columns) is where the tile kernel is ahead on all.
+#define T32_MIN_COLS 49
+
+bool b200_mmq_tc32_supported(int type, int64_t m, int64_t k, int64_t ncols) {
+    static const bool off = getenv("B200_MMQ_DISABLE_TC") != nullptr;     // comparison arm: column groups through the matvec kernel
+    return !off && type_is_block32(type) && m > 0 && ncols >= T32_MIN_COLS && k > 0 && k % 256 == 0;
+}
+int64_t b200_mmq_tc32_workspace(int64_t k, int64_t ncols) { return tc32_geom(k, ncols).total; }
+
+template <int T> static int tc32_launch(const Tc32Args & a, cudaStream_t st) {
+    static bool attr[64] = { false };
+    int dev = 0; cudaGetDevice(&dev);
+    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(mmq_tc32_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, Tc32Smem::TOTAL)); attr[dev & 63] = true; }
+    const int grid = a.n_tiles < b200_sm_count() ? a.n_tiles : b200_sm_count();
+    B200_CUDA(b200_launch_pdl(mmq_tc32_kernel<T>, dim3((unsigned)grid), dim3(T32_THREADS), (size_t)Tc32Smem::TOTAL, st, a));
+    b200_count_launch();
+    return B200_OK;
+}
+
+// k: length of the (padded) weight rows; k_valid <= k: elements that exist in X
+int b200_mmq_tc32(int type, const void * W, const float * X, int64_t x_col_stride, float * dst, int64_t ldd, int64_t m, int64_t k, int64_t k_valid, int64_t ncols, void * workspace, void * stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (((uintptr_t)W | (uintptr_t)X | (uintptr_t)workspace) & 15 || (x_col_stride & 3)) { b200_set_error("mul_mat_q: pointers must be 16-byte aligned"); return B200_ERR_INVALID; }
+    if (k_valid <= 0 || k_valid > k || k_valid % 8 != 0) { b200_set_error("mul_mat_q: k_valid must be a positive multiple of 8, at most k"); return B200_ERR_INVALID; }
+    const Tc32Geom g = tc32_geom(k, ncols);
+    Tc32Args a;
+    a.W = (const uint8_t *)W; a.ws = (const uint8_t *)workspace; a.dst = dst; a.m = m; a.k = k; a.ncols = ncols; a.ldd = ldd;
+    a.rb = (k / 32) * type_block_bytes(type); a.nt = g.nt; a.ns = (int32_t)g.ns;
+    a.n_tiles = (int32_t)(((m + T32_TM - 1) / T32_TM) * g.nt);
+    a.prof = b200_mmq_prof_buf();
+    dim3 qgrid((unsigned)(k / 256), (unsigned)(g.nt * 16));
+    B200_CUDA(b200_launch_pdl(quantize_mmq32_kernel, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k_valid, (uint8_t *)workspace, g));
+    b200_count_launch();
+    int rc = B200_ERR_UNSUPPORTED;
+    switch (type) {
+        case B200_TYPE_Q4_0: rc = tc32_launch<B200_TYPE_Q4_0>(a, st); break;
+        case B200_TYPE_Q5_0: rc = tc32_launch<B200_TYPE_Q5_0>(a, st); break;
+        case B200_TYPE_Q8_0: rc = tc32_launch<B200_TYPE_Q8_0>(a, st); break;
+    }
+    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc32", type, m, k, ncols, a.n_tiles, st);
+    return rc;
+}

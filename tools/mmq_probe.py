@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Bring-up aid for the wgmma batched MUL_MAT (mmq_tc.cu): one shape, error statistics against the C oracle, sample values."""
+"""Bring-up aid for the wgmma batched MUL_MAT (mmq_tc.cu, mmq_tc32.cu): one shape, error statistics against the C oracle, sample values."""
 import os
 import sys
 
@@ -9,10 +9,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from conftest import load_pkg  # noqa: E402
-from refutil import Q4_K, Q5_K, Q6_K, orc_mul_mat, rand_blocks  # noqa: E402
+from refutil import Q4_0, Q5_0, Q8_0, Q4_K, Q5_K, Q6_K, orc_mul_mat, rand_blocks  # noqa: E402
 
 b = load_pkg().ops
-T = {"q4_K": Q4_K, "q5_K": Q5_K, "q6_K": Q6_K}[sys.argv[1] if len(sys.argv) > 1 else "q4_K"]
+T = {"q4_K": Q4_K, "q5_K": Q5_K, "q6_K": Q6_K, "q4_0": Q4_0, "q5_0": Q5_0, "q8_0": Q8_0}[sys.argv[1] if len(sys.argv) > 1 else "q4_K"]
 m, k, n = (int(v) for v in (sys.argv[2:5] if len(sys.argv) > 4 else (128, 2048, 128)))
 rng = np.random.default_rng(3)
 W = rand_blocks(rng, T, m, k)

@@ -1,6 +1,8 @@
 #!/usr/bin/env python3
-"""Prefill tok/s through the product path (libllama + libggml-b200.so, in-process): Llama-3-8B Q4_K_M synthetic GGUF,
-a 4096-token prompt in 512-token ubatches (BASELINE config 3) and the first 512-token ubatch alone; F16 and Q8_0 KV."""
+"""Prefill tok/s through the product path (libllama + libggml-b200.so, in-process) on a synthetic GGUF (--config / --ftype,
+default Llama-3-8B Q4_K_M): a 4096-token prompt in 512-token ubatches (BASELINE config 3) and the first 512-token ubatch alone;
+F16 and Q8_0 KV.  B200_MMQ_DISABLE_TC=1 in the environment times the column-group arm of the batched MUL_MAT."""
+import argparse
 import os
 import subprocess
 import sys
@@ -12,9 +14,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from drvutil import Drv  # noqa: E402
 
-path = "/dev/shm/b200_bench_llama3-8b_Q4_K_M.gguf"
+ap = argparse.ArgumentParser()
+ap.add_argument("--config", default="llama3-8b"); ap.add_argument("--ftype", default="Q4_K_M")
+args = ap.parse_args()
+path = f"/dev/shm/b200_bench_{args.config}_{args.ftype}.gguf"
 if not os.path.exists(path):
-    subprocess.run([sys.executable, os.path.join(ROOT, "oracle", "make_gguf.py"), "--config", "llama3-8b", "--ftype", "Q4_K_M", "--out", path], check=True, capture_output=True)
+    subprocess.run([sys.executable, os.path.join(ROOT, "oracle", "make_gguf.py"), "--config", args.config, "--ftype", args.ftype, "--out", path], check=True, capture_output=True)
 rng = np.random.default_rng(1)
 for kv in ("f16", "q8_0"):
     d = Drv(path, ctx=8192, ubatch=512, ctk=kv, ctv=kv)
@@ -28,5 +33,5 @@ for kv in ("f16", "q8_0"):
         d.logits()
         res[n] = n / (time.perf_counter() - t0)
         d.reset()
-    print(f"kv {kv}: pp512 {res[512]:.0f} tok/s, pp4096 {res[4096]:.0f} tok/s  (tc attention {'off' if os.environ.get('B200_FATTN_DISABLE_TC') else 'on'})")
+    print(f"{args.config} {args.ftype} (batched MUL_MAT: {'column groups' if os.environ.get('B200_MMQ_DISABLE_TC') else 'tensor cores'}) kv {kv}: pp512 {res[512]:.0f} tok/s, pp4096 {res[4096]:.0f} tok/s  (tc attention {'off' if os.environ.get('B200_FATTN_DISABLE_TC') else 'on'})")
     d.close()
