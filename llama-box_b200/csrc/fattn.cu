@@ -498,7 +498,7 @@ static int fa_launch(const float * q, int64_t q_ts, int64_t q_hs, const void * k
 
 bool b200_fattn_tc_supported(int kv_type, int64_t dk, int64_t dv, int64_t n_tok, int64_t n_kv, float max_bias);
 int  b200_fattn_tc(const float * q, int64_t q_ts, int64_t q_hs, const void * k, int64_t k_rs, int64_t k_hs, const void * v, int64_t v_rs, int64_t v_hs,
-                   const void * mask, int64_t mask_rs, float * dst, int kv_type, int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv,
+                   const void * mask, int64_t mask_rs, float * dst, int kv_type, int64_t d, int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv,
                    float scale, float softcap, void * stream);
 
 static int fa_dispatch(const float * q, int64_t q_ts, int64_t q_hs, const void * k, int64_t k_rs, int64_t k_hs,
@@ -512,10 +512,12 @@ static int fa_dispatch(const float * q, int64_t q_ts, int64_t q_hs, const void *
     if (((uintptr_t)q & 15) || (q_ts & 3) || (q_hs & 3)) { b200_set_error("flash_attn: q must be 16-byte aligned"); return B200_ERR_INVALID; }
     if (kv_type == B200_TYPE_F16 && ((((uintptr_t)k | (uintptr_t)v) & 15) || ((k_rs | k_hs | v_rs | v_hs) & 15))) { b200_set_error("flash_attn: f16 K/V rows must be 16-byte aligned"); return B200_ERR_INVALID; }
     if (n_tok > 65535) { b200_set_error("flash_attn: n_tok * n_head too large for one launch"); return B200_ERR_UNSUPPORTED; }
-    // multi-token batches (prefill, big verify batches): the tensor-core kernel (fattn_tc.cu) — K / V read once per 128 query tokens
+    // multi-token batches (prefill, big verify batches): the tensor-core kernel (fattn_tc.cu) — K / V read once per 128 query tokens.
+    // Head 128 from 16 tokens, head 64 from the minimum its sweep measured (FT_MIN_TOK_D64); fewer tokens (speculative verify
+    // batches), the fused decode launch and ALiBi stay on the vector kernel below
     if (!fu.enabled && b200_fattn_tc_supported(kv_type, dk, dv, n_tok, n_kv, max_bias) && (!mask || ((mask_rs & 7) == 0 && ((uintptr_t)mask & 15) == 0)) &&
         (kv_type != B200_TYPE_F16 || (((k_rs | k_hs | v_rs | v_hs) & 15) == 0)))
-        return b200_fattn_tc(q, q_ts, q_hs, k, k_rs, k_hs, v, v_rs, v_hs, mask, mask_rs, dst, kv_type, n_head, n_head_kv, n_tok, n_kv, scale, softcap, stream);
+        return b200_fattn_tc(q, q_ts, q_hs, k, k_rs, k_hs, v, v_rs, v_hs, mask, mask_rs, dst, kv_type, dk, n_head, n_head_kv, n_tok, n_kv, scale, softcap, stream);
     const int64_t gq = n_head / n_head_kv;
     // query heads per CTA.  G = 4 halves the K/V reads from L2 but leaves half as many CTAs to keep loads in flight: on an H100 SXM
     // (400 W) Llama-3-8B decode ran 407 tok/s with G = 4 (8 tiles x 16 splits, one CTA per SM) and 415 tok/s with G = 2 (16 x 16)

@@ -1,6 +1,6 @@
 // fattn_tc.cu — FLASH_ATTN_EXT for multi-token batches (prefill, large verify batches) on the Hopper tensor cores (sm_90a):
-// both contractions (S = Q K^T and O = P V) are wgmma m64n128k16 f16 with f32 register accumulators, softmax runs online in
-// registers.
+// both contractions (S = Q K^T and O = P V) are wgmma f16 with f32 register accumulators, softmax runs online in registers.
+// Two instances, head size D = 128 and D = 64: S is m64n128 either way (D / 16 MMAs of K = 16), O = P V is m64n<D>k16.
 //
 // Replaces the multi-token path of ggml_cuda_flash_attn_ext: flash_attn_ext_f16 (ggml-cuda/fattn-mma-f16.cuh:395-1410, mma.sync
 // tiles, after a to_fp16 expansion of the WHOLE cache: fattn-common.cuh:780-833) — here K / V rows are read from the cache in
@@ -10,7 +10,7 @@
 //     loader warps   K, V rows (f16, or q8_0 de-quantised to f16 d*q) -> shared memory as core matrices.  Both tiles have the
 //                    same image [d / 8][position][8 halves]: for S = Q K^T it is the K-major B operand, for O = P V the SAME image
 //                    is an MN-major B operand (n = d, k = position), so V needs no transposition at all
-//     consumers      two warpgroups, 64 query rows each: S[64 q][128 kv] = Q K^T (8 x wgmma, K = 16 over d) into registers;
+//     consumers      two warpgroups, 64 query rows each: S[64 q][128 kv] = Q K^T (D / 16 x wgmma, K = 16 over d) into registers;
 //                    s * scale + mask, online max / sum in f32 (ggml-cpu/ops.cpp:8252-8404 semantics); P = exp(s - m) rounded
 //                    to f16 straight from the S registers into the A-operand registers of O = O * alpha + P V (8 x wgmma,
 //                    K = 16 over positions); the running O stays in the accumulator registers
@@ -37,8 +37,10 @@ struct FtArgs {
     float scale, softcap;
 };
 
-struct FtSmem {
-    static constexpr int Q = 0, K = 32768, V = K + 2 * 32768, BAR = V + 2 * 32768, TOTAL = BAR + 256;
+// Q tile, then two K and two V stages: each [D / 8][128 rows][16 bytes] (32 KB at D = 128, 16 KB at D = 64)
+template <int D> struct FtSmem {
+    static constexpr int TILE = D / 8 * FT_PANEL;
+    static constexpr int Q = 0, K = TILE, V = K + 2 * TILE, BAR = V + 2 * TILE, TOTAL = BAR + 256;
 };
 
 __device__ __forceinline__ void ft_fence_async()  { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -62,9 +64,11 @@ __device__ __forceinline__ uint4 kv_chunk(const uint8_t * row, int c) {
     return r;
 }
 
-template <int KVT>
+template <int D, int KVT>
 __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_constant__ FtArgs a) {
-    constexpr int D = 128;
+    static_assert(D == 64 || D == 128, "head size");
+    using FtSmem = ::FtSmem<D>;
+    constexpr int NC = D / 8;                                   // 16-byte K-chunks of a head row = core-matrix panels of a tile
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t * bars = (uint64_t *)(smem + FtSmem::BAR);
     // kv_full[2]: K,V stage loaded (3 loader warp arrivals) | kv_empty[2]: both consumer warpgroups done with the stage
@@ -121,7 +125,7 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
             uint8_t * Qs = smem + FtSmem::Q + t * 16;
             const float * qp = a.q + (int64_t)(tok < a.n_tok ? tok : 0) * a.q_ts + (int64_t)h * a.q_hs;
 #pragma unroll
-            for (int c = 0; c < 16; c++) {
+            for (int c = 0; c < NC; c++) {
                 uint4 o = make_uint4(0, 0, 0, 0);
                 if (tok < a.n_tok) {
                     const float4 x = *(const float4 *)(qp + c * 8), y = *(const float4 *)(qp + c * 8 + 4);
@@ -141,9 +145,9 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
             const bool in = p < a.n_kv;
             const uint8_t * krow = a.k + (int64_t)(in ? p : 0) * a.k_rs + (int64_t)hk * a.k_hs;
             const uint8_t * vrow = a.v + (int64_t)(in ? p : 0) * a.v_rs + (int64_t)hk * a.v_hs;
-            uint8_t * Ks = smem + FtSmem::K + st * 32768 + t * 16, * Vs = smem + FtSmem::V + st * 32768 + t * 16;
+            uint8_t * Ks = smem + FtSmem::K + st * FtSmem::TILE + t * 16, * Vs = smem + FtSmem::V + st * FtSmem::TILE + t * 16;
 #pragma unroll 4
-            for (int c = 0; c < 16; c++) {
+            for (int c = 0; c < NC; c++) {
                 uint4 kk = make_uint4(0, 0, 0, 0), vv = kk;
                 if (in) { kk = kv_chunk<KVT>(krow, c); vv = kv_chunk<KVT>(vrow, c); }
                 *(uint4 *)(Ks + c * FT_PANEL) = kk;
@@ -167,9 +171,9 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
             row_ok[u] = tok < a.n_tok;
             mrow[u] = a.mask ? a.mask + (int64_t)(row_ok[u] ? tok : 0) * a.mask_rs : nullptr;
         }
-        float O[64], S[64];
+        float O[D / 2], S[64];                                                 // O: m64 x n<D> accumulator, S: m64 x n128
 #pragma unroll
-        for (int c = 0; c < 64; c++) O[c] = 0.0f;
+        for (int c = 0; c < D / 2; c++) O[c] = 0.0f;
         float M[2] = { -INFINITY, -INFINITY }, L[2] = { 0.0f, 0.0f };           // L: this thread's share of the row sum
         const float scale = a.softcap != 0.0f ? a.scale / a.softcap : a.scale;
         const uint32_t qs = smem_u32(smem + FtSmem::Q) + g * 1024;
@@ -178,10 +182,10 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
             const int st = i & 1;
             const int pb = s_blocks[i] * 128;
             mbar_wait(&kv_full[st], (i >> 1) & 1);
-            const uint32_t ks = smem_u32(smem + FtSmem::K + st * 32768), vs = smem_u32(smem + FtSmem::V + st * 32768);
+            const uint32_t ks = smem_u32(smem + FtSmem::K + st * FtSmem::TILE), vs = smem_u32(smem + FtSmem::V + st * FtSmem::TILE);
             wg_fence();
 #pragma unroll
-            for (int j = 0; j < 8; j++) wg_mma_ss(S, wg_desc(qs + j * 2 * FT_PANEL, FT_PANEL, 128), wg_desc(ks + j * 2 * FT_PANEL, FT_PANEL, 128), j ? 1u : 0u);
+            for (int j = 0; j < NC / 2; j++) wg_mma_ss(S, wg_desc(qs + j * 2 * FT_PANEL, FT_PANEL, 128), wg_desc(ks + j * 2 * FT_PANEL, FT_PANEL, 128), j ? 1u : 0u);
             wg_commit();
             wg_wait0();
             wg_pin(S);
@@ -231,7 +235,7 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
                 }
             }
 #pragma unroll
-            for (int j = 0; j < 16; j++) {
+            for (int j = 0; j < NC; j++) {
 #pragma unroll
                 for (int u = 0; u < 2; u++) { O[4 * j + 2 * u] *= alpha[u]; O[4 * j + 2 * u + 1] *= alpha[u]; }
             }
@@ -256,30 +260,37 @@ __global__ void __launch_bounds__(FT_THREADS, 1) fattn_tc_kernel(const __grid_co
             const float inv = l > 0.0f ? 1.0f / l : 0.0f;                        // ops.cpp:8390-8392 (V /= S)
             float * out = a.dst + ((int64_t)(q0 + ra + 8 * u) * a.n_head + h) * D;
 #pragma unroll
-            for (int j = 0; j < 16; j++) *(float2 *)(out + 8 * j + c0) = make_float2(O[4 * j + 2 * u] * inv, O[4 * j + 2 * u + 1] * inv);
+            for (int j = 0; j < NC; j++) *(float2 *)(out + 8 * j + c0) = make_float2(O[4 * j + 2 * u] * inv, O[4 * j + 2 * u + 1] * inv);
         }
     }
     pdl_trigger();
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
+// Fewest query tokens per head size for which this kernel beats the vector kernel (fattn.cu), which reads K / V once per token.
+// Head 64 from a sweep of both arms (tools/fattn_bench.py --sweep, H100.md): at 32 tokens the vector kernel is still ahead on a
+// Q8_0 cache, from 40 on this kernel wins or ties on both cache types.
+#define FT_MIN_TOK_D128 16
+#define FT_MIN_TOK_D64 40
+
 bool b200_fattn_tc_supported(int kv_type, int64_t dk, int64_t dv, int64_t n_tok, int64_t n_kv, float max_bias) {
     static const bool off = getenv("B200_FATTN_DISABLE_TC") != nullptr;
-    return !off && dk == 128 && dv == 128 && n_tok >= 16 && n_kv % 8 == 0 && n_kv <= 512 * 128 && max_bias == 0.0f && (kv_type == B200_TYPE_F16 || kv_type == B200_TYPE_Q8_0);
+    const bool shape = (dk == 128 && dv == 128 && n_tok >= FT_MIN_TOK_D128) || (dk == 64 && dv == 64 && n_tok >= FT_MIN_TOK_D64);
+    return !off && shape && n_kv % 8 == 0 && n_kv <= 512 * 128 && max_bias == 0.0f && (kv_type == B200_TYPE_F16 || kv_type == B200_TYPE_Q8_0);
 }
 
-template <int KVT> static int ft_launch(const FtArgs & a, cudaStream_t st) {
+template <int D, int KVT> static int ft_launch(const FtArgs & a, cudaStream_t st) {
     static bool attr[64] = { false };
     int dev = 0; cudaGetDevice(&dev);
-    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(fattn_tc_kernel<KVT>, cudaFuncAttributeMaxDynamicSharedMemorySize, FtSmem::TOTAL)); attr[dev & 63] = true; }
+    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(fattn_tc_kernel<D, KVT>, cudaFuncAttributeMaxDynamicSharedMemorySize, FtSmem<D>::TOTAL)); attr[dev & 63] = true; }
     dim3 grid((unsigned)((a.n_tok + 127) / 128), (unsigned)a.n_head);
-    B200_CUDA(b200_launch_pdl(fattn_tc_kernel<KVT>, grid, dim3(FT_THREADS), (size_t)FtSmem::TOTAL, st, a));
+    B200_CUDA(b200_launch_pdl(fattn_tc_kernel<D, KVT>, grid, dim3(FT_THREADS), (size_t)FtSmem<D>::TOTAL, st, a));
     b200_count_launch();
     return B200_OK;
 }
 
 int b200_fattn_tc(const float * q, int64_t q_ts, int64_t q_hs, const void * k, int64_t k_rs, int64_t k_hs, const void * v, int64_t v_rs, int64_t v_hs,
-                  const void * mask, int64_t mask_rs, float * dst, int kv_type, int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv,
+                  const void * mask, int64_t mask_rs, float * dst, int kv_type, int64_t d, int64_t n_head, int64_t n_head_kv, int64_t n_tok, int64_t n_kv,
                   float scale, float softcap, void * stream) {
     FtArgs a;
     a.q = q; a.q_ts = q_ts; a.q_hs = q_hs; a.k = (const uint8_t *)k; a.k_rs = k_rs; a.k_hs = k_hs; a.v = (const uint8_t *)v; a.v_rs = v_rs; a.v_hs = v_hs;
@@ -287,5 +298,9 @@ int b200_fattn_tc(const float * q, int64_t q_ts, int64_t q_hs, const void * k, i
     a.n_head = (int32_t)n_head; a.n_head_kv = (int32_t)n_head_kv; a.n_tok = (int32_t)n_tok; a.n_kv = (int32_t)n_kv; a.kv_type = kv_type;
     a.scale = scale; a.softcap = softcap;
     if (mask && ((mask_rs & 7) || ((uintptr_t)mask & 15))) { b200_set_error("flash_attn (tensor core): mask rows must be 16-byte aligned"); return B200_ERR_INVALID; }
-    return kv_type == B200_TYPE_F16 ? ft_launch<B200_TYPE_F16>(a, (cudaStream_t)stream) : ft_launch<B200_TYPE_Q8_0>(a, (cudaStream_t)stream);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (d == 128) return kv_type == B200_TYPE_F16 ? ft_launch<128, B200_TYPE_F16>(a, st) : ft_launch<128, B200_TYPE_Q8_0>(a, st);
+    if (d == 64)  return kv_type == B200_TYPE_F16 ? ft_launch<64, B200_TYPE_F16>(a, st) : ft_launch<64, B200_TYPE_Q8_0>(a, st);
+    b200_set_error("flash_attn (tensor core): head size %lld unsupported (64 or 128)", (long long)d);
+    return B200_ERR_UNSUPPORTED;
 }

@@ -1,5 +1,7 @@
 #!/usr/bin/env python3
-"""Bring-up aid for fattn_tc.cu: one multi-token attention shape against an f64 evaluation; error statistics per query tile / head."""
+"""Bring-up aid for fattn_tc.cu: one multi-token attention shape against an f64 evaluation; error statistics per query tile / head.
+
+    fattn_probe.py f16|q8_0 n_head n_head_kv n_tok n_kv past [head_size, default 128]"""
 import os
 import sys
 
@@ -14,7 +16,7 @@ from refutil import F16, Q8_0, oracle, orc_dequant, ptr, row_bytes  # noqa: E402
 b = load_pkg().ops
 kvt = {"f16": F16, "q8_0": Q8_0}[sys.argv[1]]
 nh, nhkv, nt, nkv, past = (int(v) for v in sys.argv[2:7])
-dk = 128
+dk = int(sys.argv[7]) if len(sys.argv) > 7 else 128
 rng = np.random.default_rng(1)
 q = rng.standard_normal((nt, nh, dk)).astype(np.float32)
 kf = rng.standard_normal((nkv, nhkv * dk)).astype(np.float32); vf = rng.standard_normal((nkv, nhkv * dk)).astype(np.float32)
@@ -47,7 +49,7 @@ for h in range(nh):
     p = np.exp(s - s.max(axis=1, keepdims=True))
     truth[:, h] = (p @ Vd[:, hk]) / p.sum(axis=1, keepdims=True)
 err = np.abs(got - truth) / np.abs(truth).max()
-print(f"{sys.argv[1]} nh={nh} nhkv={nhkv} nt={nt} nkv={nkv} past={past}: finite {np.isfinite(got).mean():.3f} max err {np.nanmax(err):.3e}")
+print(f"{sys.argv[1]} D={dk} nh={nh} nhkv={nhkv} nt={nt} nkv={nkv} past={past}: finite {np.isfinite(got).mean():.3f} max err {np.nanmax(err):.3e}")
 for t0 in range(0, nt, 128):
     e = err[t0:t0 + 128]
     print(f"  q tile {t0 // 128}: max err {np.nanmax(e):.2e}; per head", " ".join(f"{np.nanmax(e[:, h]):.1e}" for h in range(min(nh, 8))), "| worst rows", np.argsort(-np.nanmax(e, axis=(1, 2)))[:5] + t0)
