@@ -193,6 +193,15 @@ B200_API int b200_mul_mat_vec_wide(int type, const void *W, const float *x, int6
 B200_API int b200_mul_mat_id(int type, const void *as, int64_t expert_stride_bytes, const float *b, int64_t b_tok_stride, int64_t b_slot_stride, int64_t n_b1,
                              const int32_t *ids, int64_t ids_tok_stride, float *dst, int64_t dst_tok_stride, int64_t dst_slot_stride,
                              int64_t m, int64_t k, int64_t n_expert, int64_t n_used, int64_t n_tok, void *stream);
+/* ... for prefill: with n_tok >= MMID_MIN_TOK and n_tok * n_used >= MMID_MIN_PAIRS * n_expert (csrc/mmid_route.cu) on Q4_0 / Q5_0 / Q8_0 / Q4_K / Q5_K / Q6_K experts (k % 256 == 0; Q6_K
+ * k % 2048 == 0) a grouped GEMM on the tensor cores: the (token, slot) pairs are grouped by expert ON THE DEVICE (no host synchronisation,
+ * capturable into a CUDA graph; replaces ggml-cuda/mmq.cu:149-193) and each expert's columns run through the tile kernel of b200_mul_mat_q,
+ * with the same results bit for bit.  `workspace` (256-byte aligned) must hold b200_mul_mat_id_workspace(...) bytes; when that is 0
+ * (other types and shapes, fewer tokens, B200_MMQ_DISABLE_TC=1) the call is b200_mul_mat_id and the workspace may be NULL. */
+B200_API int64_t b200_mul_mat_id_workspace(int type, int64_t m, int64_t k, int64_t n_expert, int64_t n_used, int64_t n_tok);
+B200_API int b200_mul_mat_id2(int type, const void *as, int64_t expert_stride_bytes, const float *b, int64_t b_tok_stride, int64_t b_slot_stride, int64_t n_b1,
+                              const int32_t *ids, int64_t ids_tok_stride, float *dst, int64_t dst_tok_stride, int64_t dst_slot_stride,
+                              int64_t m, int64_t k, int64_t n_expert, int64_t n_used, int64_t n_tok, void *workspace, void *stream);
 /* GET_ROWS on a quantised table: dst row i = de-quantised row ids[i] of src (replaces k_get_rows, ggml-cuda/getrows.cu:5-67; values
  * bit-identical to ggml's dequantize_row_*: products rounded separately).  The token-embedding lookup on the device. */
 B200_API int b200_get_rows_q(int type, const void *src, int64_t src_row_stride_bytes, int64_t nrows, const int32_t *ids, float *dst,

@@ -945,11 +945,18 @@ struct Runner {
                 invalidate_act(n.dst);
                 return KL(b200_sum_rows((const float *)n.src[0].data, n.src[0].ne[0], (float *)n.dst.data, n.src[0].ne[0], nrows_of(n.src[0]), st));
             case B200_OP_MUL_MAT_ID: {
-                // expert routing on the device: the kernel reads ids itself (no stream synchronisation, unlike ggml-cuda.cu:2115-2125)
+                // expert routing on the device: the kernels read ids themselves (no stream synchronisation, unlike ggml-cuda.cu:2115-2125)
                 invalidate_act(n.dst);
                 const b200_tensor & w = n.src[0], & x = n.src[1], & ids = n.src[2];
-                return KL(b200_mul_mat_id(w.type, w.data, w.nb[2], (const float *)x.data, x.nb[2] / 4, x.nb[1] / 4, x.ne[1], (const int32_t *)ids.data, ids.nb[1] / 4,
-                                          (float *)n.dst.data, n.dst.nb[2] / 4, n.dst.nb[1] / 4, w.ne[1], w.ne[0], w.ne[2], ids.ne[0], ids.ne[1], st));
+                const bool grouped = b200_mul_mat_id_workspace(w.type, w.ne[1], w.ne[0], w.ne[2], ids.ne[0], ids.ne[1]) > 0;
+                uint8_t * ws = nullptr;
+                if (grouped) {                                 // prefill: the grouped GEMM builds its schedule and activation image in the act buffer
+                    { const int fs = mk_flush(); if (fs != B200_OK) return fs; }
+                    ex->act_id[0] = ex->act_id[1] = 0;
+                    ws = act_buf(b200_act_kind_for(w.type));
+                }
+                return KL(b200_mul_mat_id2(w.type, w.data, w.nb[2], (const float *)x.data, x.nb[2] / 4, x.nb[1] / 4, x.ne[1], (const int32_t *)ids.data, ids.nb[1] / 4,
+                                           (float *)n.dst.data, n.dst.nb[2] / 4, n.dst.nb[1] / 4, w.ne[1], w.ne[0], w.ne[2], ids.ne[0], ids.ne[1], ws, st));
             }
             case B200_OP_GET_ROWS:
                 invalidate_act(n.dst);
@@ -1016,6 +1023,10 @@ int plan_workspace(b200_executor * ex, const b200_node * nodes, int n) {
                 const size_t b = (size_t)b200_mul_mat_q_workspace(nd.src[0].type, nd.src[0].ne[1], k, cols);
                 if (kd >= 0 && b > act[kd]) act[kd] = b;
             }
+        } else if (nd.op == B200_OP_MUL_MAT_ID && nd.n_src >= 3) {   // grouped GEMM of a prefill: schedule + activation image
+            const int kd = b200_act_kind_for(nd.src[0].type);
+            const size_t b = (size_t)b200_mul_mat_id_workspace(nd.src[0].type, nd.src[0].ne[1], nd.src[0].ne[0], nd.src[0].ne[2], nd.src[2].ne[0], nd.src[2].ne[1]);
+            if (kd >= 0 && b > act[kd]) act[kd] = b;
         } else if (nd.op == B200_OP_RMS_NORM) {
             for (int kd = 0; kd < 2; kd++) { const size_t b = (size_t)(8 * act_col_bytes(kd, (nd.src[0].ne[0] + 255) / 256 * 256)); if (b > act[kd]) act[kd] = b; }
         } else if (nd.op == B200_OP_FLASH_ATTN_EXT) {

@@ -34,6 +34,7 @@
 // run on neighbouring CTAs), activations stream from L2.
 #include "common.cuh"
 #include "wgmma.cuh"
+#include "mmid.cuh"
 
 #include <cuda_fp16.h>
 #include <cstdio>
@@ -64,15 +65,27 @@ static TcGeom tc_geom(int64_t k, int64_t ncols) {
 // ---- activation quantisation into the B image -------------------------------------------------------------------------
 // one warp per (token, super-block); exactly quantize_row_q8_K_ref: first index of the largest |x|, iscale = -127/max,
 // nearest-int (RNE), MIN(127, .), d = 1/iscale, bsums per 16
+// GATHER (grouped MUL_MAT_ID, mmid.cuh): column n of the image is the pair map.cols[n] of the activation x (zeros for padding); the blocks
+// of column tiles past *map.ntt exit.  Each column's image is the one the dense instance writes for the same f32 column.
+template <bool GATHER>
 __global__ void __launch_bounds__(256) quantize_mmq_kernel(const float * __restrict__ x, int64_t x_col_stride, int64_t ncols, int64_t k,
-                                                          uint8_t * __restrict__ ws, TcGeom g) {
+                                                          uint8_t * __restrict__ ws, TcGeom g, MmidMap map) {
     pdl_wait();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t sb = blockIdx.x;
     const int64_t n = (int64_t)blockIdx.y * 8 + warp;                // token (padded range: < nt * 128)
     const int64_t nt = n >> 7; const int nl = (int)(n & 127);
     float v[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    if (n < ncols) {
+    if constexpr (GATHER) {
+        if (nt >= *map.ntt) return;                                  // the whole block: blockIdx.y / 16 is its column tile
+        const int pr = map.cols[n], nu = map.n_used;
+        if (pr >= 0) {
+            const int t = pr / nu, s = pr % nu;
+            const float4 * p = (const float4 *)(x + (int64_t)t * map.b_tok_stride + (s % map.n_b1) * map.b_slot_stride + sb * 256 + lane * 8);
+            const float4 a = p[0], b = p[1];
+            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+        }
+    } else if (n < ncols) {
         const float4 * p = (const float4 *)(x + n * x_col_stride + sb * 256 + lane * 8);
         const float4 a = p[0], b = p[1];
         v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
@@ -124,6 +137,7 @@ struct TcArgs {
     int32_t nsb, n_mtiles, n_tiles, type;
     uint32_t lbo, sbo;          // descriptor strides (bytes): K-chunk stride / 8-row-group stride
     unsigned long long * prof;  // bring-up: per-role cycle counters of CTA 0 (B200_MMQ_PROF), normally null
+    MmidMap map;                // GROUPED only: W is the first expert's matrix, columns are (token, slot) pairs
 };
 // ---- per-type pipeline geometry: K-stages per super-block, whether the mins MMA runs, activation bytes per stage -------
 // (the transform threads read each row's packed blocks straight from global memory, so no weight bytes live in shared memory;
@@ -156,7 +170,9 @@ __device__ __forceinline__ void k4_unpack(uint32_t y, uint32_t z, uint32_t w, ui
     mn47 = ((w >> 4) & 0x0f0f0f0fu) | (((z >> 6) & 0x03030303u) << 4);
 }
 
-template <int T>
+// GROUPED (MUL_MAT_ID, mmid.cuh): column tile ct multiplies expert map.tile_expert[ct]; the tile count comes from the device (*map.ntt)
+// and the epilogue scatters column j to its pair's output row (padding columns are not stored).  Everything else is the dense kernel.
+template <int T, bool GROUPED>
 __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_constant__ TcArgs args) {
     using TT = TcType<T>;
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -172,7 +188,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
     pdl_wait();
 
     const int nsb = args.nsb;
-    const int64_t NT = args.g.nt;
+    const auto NT = [&]() { if constexpr (GROUPED) return *args.map.ntt; else return args.g.nt; }();     // column tiles (grouped: 32-bit tile arithmetic)
+    auto n_tiles = [&]() { return GROUPED ? args.n_mtiles * (int)NT : args.n_tiles; };      // dense: read from the parameters at each use
     unsigned long long w0 = 0, w1 = 0, w2 = 0;                       // profile: cycles in this role's kinds of waits
     const bool prof = args.prof != nullptr && blockIdx.x == 0;
     unsigned long long * pw0 = prof ? &w0 : nullptr, * pw1 = prof ? &w1 : nullptr;
@@ -209,6 +226,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
             const int64_t m0 = (int64_t)(tile / NT) * TC_TM;
             int64_t r = m0 + t; if (r >= args.m) r = args.m - 1;             // rows past the end: any valid row (their results are never stored)
             const uint8_t * row = args.W + r * args.rb;
+            if constexpr (GROUPED) row += (int64_t)args.map.tile_expert[tile - (m0 / TC_TM) * NT] * args.map.expert_stride;   // column tile = tile % NT
             if (T == B200_TYPE_Q6_K) {
                 const uint4 * ql = (const uint4 *)(row + (int64_t)sb * 128), * qh = (const uint4 *)(row + nb * 128 + (int64_t)sb * 64);
 #pragma unroll
@@ -223,8 +241,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                 for (int i = 0; i < NW; i++) nxt[i] = __ldg(p + i);
             }
         };
-        if (blockIdx.x < args.n_tiles) fetch(blockIdx.x, 0);
-        for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
+        if (blockIdx.x < n_tiles()) fetch(blockIdx.x, 0);
+        for (int tile = blockIdx.x; tile < n_tiles(); tile += gridDim.x) {
             for (int sb = 0; sb < nsb; sb++, sbc++) {
                 const int rs = sbc & 1;                                  // accumulator / imin-operand slot
                 uint4 cur[NW]; const uint16_t cur_d = nxt_d;
@@ -233,7 +251,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                 {   // prefetch the next super-block (of this tile, or the first one of this CTA's next tile)
                     int ntile = tile, nsbi = sb + 1;
                     if (nsbi == nsb) { nsbi = 0; ntile = tile + gridDim.x; }
-                    if (ntile < args.n_tiles) fetch(ntile, nsbi);
+                    if (ntile < n_tiles()) fetch(ntile, nsbi);
                 }
                 float2 * rscale = (float2 *)(smem + TcSmem::RS + (sbc & 3) * 1024);
                 if (T == B200_TYPE_Q4_K || T == B200_TYPE_Q5_K) {
@@ -345,7 +363,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
         const int c0 = 2 * (lane & 3);                                  // tile columns 8 j + c0 + {0, 1}
         const uint64_t dmin_a = wg_desc(smem_u32(smem + TcSmem::AM + g * 1024), args.lbo, args.sbo);
         uint32_t it = 0, sbc = 0;
-        for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
+        for (int tile = blockIdx.x; tile < n_tiles(); tile += gridDim.x) {
             const int64_t mt = tile / NT, nt = tile % NT;
             float acc[64], frag[64];
 #pragma unroll
@@ -409,7 +427,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
                         const int64_t n = nt * TC_TN + 8 * j + c0 + e;
-                        if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
+                        if constexpr (GROUPED) {
+                            const int pr = args.map.cols[n], nu = args.map.n_used;
+                            if (pr >= 0) args.dst[(pr / nu) * args.map.dst_tok_stride + (pr % nu) * args.map.dst_slot_stride + row] = acc[4 * j + 2 * h + e];
+                        } else if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
                     }
                 }
             }
@@ -436,12 +457,13 @@ bool b200_mmq_tc_supported(int type, int64_t m, int64_t k, int64_t ncols) {
 }
 int64_t b200_mmq_tc_workspace(int64_t k, int64_t ncols) { return tc_geom(k, ncols).total; }
 
-template <int T> static int tc_launch(const TcArgs & a, cudaStream_t st) {
+// grouped: a.n_tiles is the host's upper bound (the kernel reads the real count)
+template <int T, bool GROUPED = false> static int tc_launch(const TcArgs & a, cudaStream_t st) {
     static bool attr[64] = { false };
     int dev = 0; cudaGetDevice(&dev);
-    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(mmq_tc_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem::TOTAL)); attr[dev & 63] = true; }
+    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(mmq_tc_kernel<T, GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem::TOTAL)); attr[dev & 63] = true; }
     int grid = a.n_tiles < b200_sm_count() ? a.n_tiles : b200_sm_count();
-    B200_CUDA(b200_launch_pdl(mmq_tc_kernel<T>, dim3((unsigned)grid), dim3(TC_THREADS), (size_t)TcSmem::TOTAL, st, a));
+    B200_CUDA(b200_launch_pdl(mmq_tc_kernel<T, GROUPED>, dim3((unsigned)grid), dim3(TC_THREADS), (size_t)TcSmem::TOTAL, st, a));
     b200_count_launch();
     return B200_OK;
 }
@@ -449,7 +471,7 @@ template <int T> static int tc_launch(const TcArgs & a, cudaStream_t st) {
 int b200_mmq_tc(int type, const void * W, const float * X, int64_t x_col_stride, float * dst, int64_t ldd, int64_t m, int64_t k, int64_t ncols, void * workspace, void * stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if (((uintptr_t)W | (uintptr_t)X | (uintptr_t)workspace) & 15 || (x_col_stride & 3)) { b200_set_error("mul_mat_q: pointers must be 16-byte aligned"); return B200_ERR_INVALID; }
-    TcArgs a;
+    TcArgs a = {};
     a.W = (const uint8_t *)W; a.ws = (const uint8_t *)workspace; a.dst = dst; a.m = m; a.k = k; a.ncols = ncols; a.ldd = ldd;
     a.rb = (k / 256) * type_block_bytes(type);
     a.g = tc_geom(k, ncols);
@@ -457,7 +479,7 @@ int b200_mmq_tc(int type, const void * W, const float * X, int64_t x_col_stride,
     a.prof = b200_mmq_prof_buf();
     a.nsb = (int32_t)(k / 256); a.n_mtiles = (int32_t)((m + TC_TM - 1) / TC_TM); a.n_tiles = (int32_t)(a.n_mtiles * a.g.nt); a.type = type;
     dim3 qgrid((unsigned)a.nsb, (unsigned)(a.g.nt * 16));
-    B200_CUDA(b200_launch_pdl(quantize_mmq_kernel, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k, (uint8_t *)workspace, a.g));
+    B200_CUDA(b200_launch_pdl(quantize_mmq_kernel<false>, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k, (uint8_t *)workspace, a.g, MmidMap{}));
     b200_count_launch();
     int rc = B200_ERR_UNSUPPORTED;
     switch (type) {
@@ -466,6 +488,30 @@ int b200_mmq_tc(int type, const void * W, const float * X, int64_t x_col_stride,
         case B200_TYPE_Q6_K: rc = tc_launch<B200_TYPE_Q6_K>(a, st); break;
     }
     if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc", type, m, k, ncols, a.n_tiles, st);
+    return rc;
+}
+
+// grouped MUL_MAT_ID (mmid_route.cu): B f32 activations gathered through map, W the first expert, n_ct the upper bound of column tiles;
+// `image` (16-byte aligned) holds b200_mmq_tc_workspace(k, 128 * n_ct) bytes
+int b200_mmq_tc_grouped(int type, const void * W, const float * B, float * dst, int64_t m, int64_t k, int64_t n_ct, const MmidMap & map, void * image, cudaStream_t st) {
+    TcArgs a = {};
+    a.W = (const uint8_t *)W; a.ws = (const uint8_t *)image; a.dst = dst; a.m = m; a.k = k; a.ncols = n_ct * TC_TN;
+    a.rb = (k / 256) * type_block_bytes(type);
+    a.g = tc_geom(k, a.ncols);
+    a.lbo = (uint32_t)TC_PANEL; a.sbo = 128u;
+    a.prof = b200_mmq_prof_buf();
+    a.nsb = (int32_t)(k / 256); a.n_mtiles = (int32_t)((m + TC_TM - 1) / TC_TM); a.n_tiles = (int32_t)(a.n_mtiles * n_ct); a.type = type;
+    a.map = map;
+    dim3 qgrid((unsigned)a.nsb, (unsigned)(n_ct * 16));
+    B200_CUDA(b200_launch_pdl(quantize_mmq_kernel<true>, qgrid, dim3(256), 0, st, B, (int64_t)0, a.ncols, k, (uint8_t *)image, a.g, map));
+    b200_count_launch();
+    int rc = B200_ERR_UNSUPPORTED;
+    switch (type) {
+        case B200_TYPE_Q4_K: rc = tc_launch<B200_TYPE_Q4_K, true>(a, st); break;
+        case B200_TYPE_Q5_K: rc = tc_launch<B200_TYPE_Q5_K, true>(a, st); break;
+        case B200_TYPE_Q6_K: rc = tc_launch<B200_TYPE_Q6_K, true>(a, st); break;
+    }
+    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc grouped", type, m, k, a.ncols, a.n_tiles, st);
     return rc;
 }
 

@@ -31,6 +31,7 @@
 // A stage is 128 k (4 blocks): A 16 KB (int8 core matrices) + B 16 KB + d_x 2 KB + d_w 2 KB; 4 stages, ~144 KB of shared memory.
 #include "common.cuh"
 #include "wgmma.cuh"
+#include "mmid.cuh"
 
 #include <cstdlib>
 
@@ -62,15 +63,27 @@ static Tc32Geom tc32_geom(int64_t k, int64_t ncols) {
 // ---- activation quantisation into the image ------------------------------------------------------------------------------
 // one warp per (token, 256 elements), 4 lanes per q8_0 block: the arithmetic of warp_quant_q80 (actquant.cuh).  Elements from
 // k_valid up (padded weight rows) and tokens from ncols up are zeros with d = 0.
+// GATHER (grouped MUL_MAT_ID, mmid.cuh): column n of the image is the pair map.cols[n] of x (zeros for padding); the blocks of column
+// tiles past *map.ntt exit.  Each column's image is the one the dense instance writes for the same f32 column.
+template <bool GATHER>
 __global__ void __launch_bounds__(256) quantize_mmq32_kernel(const float * __restrict__ x, int64_t x_col_stride, int64_t ncols, int64_t k_valid,
-                                                            uint8_t * __restrict__ ws, Tc32Geom g) {
+                                                            uint8_t * __restrict__ ws, Tc32Geom g, MmidMap map) {
     pdl_wait();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t blk = blockIdx.x;
     const int64_t n = (int64_t)blockIdx.y * 8 + warp;                // token (padded range: < nt * 128)
     const int64_t nt = n >> 7; const int nl = (int)(n & 127);
     float v[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    if (n < ncols && blk * 256 + lane * 8 < k_valid) {
+    if constexpr (GATHER) {
+        if (nt >= *map.ntt) return;                                  // the whole block: blockIdx.y / 16 is its column tile
+        const int pr = map.cols[n], nu = map.n_used;
+        if (pr >= 0) {
+            const int t = pr / nu, s = pr % nu;
+            const float4 * p = (const float4 *)(x + (int64_t)t * map.b_tok_stride + (s % map.n_b1) * map.b_slot_stride + blk * 256 + lane * 8);
+            const float4 a = p[0], b = p[1];
+            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+        }
+    } else if (n < ncols && blk * 256 + lane * 8 < k_valid) {
         const float4 * p = (const float4 *)(x + n * x_col_stride + blk * 256 + lane * 8);
         const float4 a = p[0], b = p[1];
         v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
@@ -102,6 +115,8 @@ struct Tc32Args {
     int64_t m, k, ncols, ldd, rb, nt;
     int32_t ns, n_tiles;
     unsigned long long * prof;  // per-role cycle counters of CTA 0 (B200_MMQ_PROF), normally null
+    MmidMap map;                // GROUPED only: W is the first expert's matrix, columns are (token, slot) pairs
+    int32_t n_mtiles;           // GROUPED only
 };
 
 struct Tc32Smem {
@@ -115,7 +130,9 @@ __device__ __forceinline__ uint32_t bit4_of(uint32_t b) { return (((b & 0xFu) * 
 // bytes v in [0, 2 OFF) -> v - OFF as int8, four at a time (no borrow crosses a byte: 0x80 + v - OFF >= 0x70)
 template <uint32_t OFF> __device__ __forceinline__ uint32_t recentre(uint32_t v) { return ((v | 0x80808080u) - OFF * 0x01010101u) ^ 0x80808080u; }
 
-template <int T>
+// GROUPED (MUL_MAT_ID, mmid.cuh): column tile ct multiplies expert map.tile_expert[ct]; the tile count comes from the device (*map.ntt)
+// and the epilogue scatters column j to its pair's output row (padding columns are not stored).  Everything else is the dense kernel.
+template <int T, bool GROUPED>
 __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_constant__ Tc32Args args) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t * b_full = (uint64_t *)(smem + Tc32Smem::BAR), * a_full = b_full + T32_NSTAGE, * ab_empty = a_full + T32_NSTAGE;
@@ -129,7 +146,8 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
     pdl_wait();
 
     const int ns = args.ns;
-    const int64_t NT = args.nt;
+    const auto NT = [&]() { if constexpr (GROUPED) return *args.map.ntt; else return args.nt; }();        // column tiles (grouped: 32-bit tile arithmetic)
+    const int n_tiles = GROUPED ? args.n_mtiles * (int)NT : args.n_tiles;
     unsigned long long w0 = 0, w1 = 0;                               // profile: cycles in this role's kinds of waits
     const bool prof = args.prof != nullptr && blockIdx.x == 0;
     unsigned long long * pw0 = prof ? &w0 : nullptr, * pw1 = prof ? &w1 : nullptr;
@@ -147,14 +165,15 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
         auto fetch = [&](int tile, int s) {
             int64_t r = (int64_t)(tile / NT) * T32_TM + t; if (r >= args.m) r = args.m - 1;   // rows past the end: any valid row (never stored)
             const uint8_t * row = args.W + r * args.rb;
+            if constexpr (GROUPED) row += (int64_t)args.map.tile_expert[tile % NT] * args.map.expert_stride;
             const uint4 * p = (const uint4 *)(row + (int64_t)s * 4 * QB);
 #pragma unroll
             for (int i = 0; i < NQ; i++) nxt[i] = __ldg(p + i);
             if (T == B200_TYPE_Q5_0) nxt_h = __ldg((const uint4 *)(row + nb * 16 + (int64_t)s * 16));
             nxt_d = __ldg((const uint2 *)(row + nb * (T == B200_TYPE_Q5_0 ? 20 : QB) + (int64_t)s * 8));
         };
-        if (blockIdx.x < args.n_tiles) fetch(blockIdx.x, 0);
-        for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
+        if (blockIdx.x < n_tiles) fetch(blockIdx.x, 0);
+        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             for (int s = 0; s < ns; s++, it++) {
                 uint4 cur[NQ]; const uint4 cur_h = nxt_h; const uint2 cur_d = nxt_d;
 #pragma unroll
@@ -162,7 +181,7 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
                 {   // prefetch the next stage (of this tile, or the first one of this CTA's next tile)
                     int ntile = tile, nsi = s + 1;
                     if (nsi == ns) { nsi = 0; ntile = tile + gridDim.x; }
-                    if (ntile < args.n_tiles) fetch(ntile, nsi);
+                    if (ntile < n_tiles) fetch(ntile, nsi);
                 }
                 const int st = it % T32_NSTAGE;
                 mbar_wait_p(&ab_empty[st], ((it / T32_NSTAGE) & 1) ^ 1, pw1);
@@ -207,7 +226,7 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
         const int ra = 64 * g + 16 * (warp & 3) + (lane >> 2);          // tile rows ra, ra + 8 (wgmma accumulator layout, wgmma.cuh)
         const int c0 = 2 * (lane & 3);                                  // tile columns 8 j + c0 + {0, 1}
         uint32_t it = 0;
-        for (int tile = blockIdx.x; tile < args.n_tiles; tile += gridDim.x) {
+        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const int64_t mt = tile / NT, nt = tile % NT;
             float acc[64];
             int32_t f0[32], f1[32];                                      // accumulators of column halves 0-63 / 64-127
@@ -271,7 +290,10 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
                         const int64_t n = nt * T32_TN + 8 * j + c0 + e;
-                        if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
+                        if constexpr (GROUPED) {
+                            const int pr = args.map.cols[n], nu = args.map.n_used;
+                            if (pr >= 0) args.dst[(pr / nu) * args.map.dst_tok_stride + (pr % nu) * args.map.dst_slot_stride + row] = acc[4 * j + 2 * h + e];
+                        } else if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
                     }
                 }
             }
@@ -298,12 +320,13 @@ bool b200_mmq_tc32_supported(int type, int64_t m, int64_t k, int64_t ncols) {
 }
 int64_t b200_mmq_tc32_workspace(int64_t k, int64_t ncols) { return tc32_geom(k, ncols).total; }
 
-template <int T> static int tc32_launch(const Tc32Args & a, cudaStream_t st) {
+// grouped: a.n_tiles is the host's upper bound (the kernel reads the real count)
+template <int T, bool GROUPED = false> static int tc32_launch(const Tc32Args & a, cudaStream_t st) {
     static bool attr[64] = { false };
     int dev = 0; cudaGetDevice(&dev);
-    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(mmq_tc32_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, Tc32Smem::TOTAL)); attr[dev & 63] = true; }
+    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(mmq_tc32_kernel<T, GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, Tc32Smem::TOTAL)); attr[dev & 63] = true; }
     const int grid = a.n_tiles < b200_sm_count() ? a.n_tiles : b200_sm_count();
-    B200_CUDA(b200_launch_pdl(mmq_tc32_kernel<T>, dim3((unsigned)grid), dim3(T32_THREADS), (size_t)Tc32Smem::TOTAL, st, a));
+    B200_CUDA(b200_launch_pdl(mmq_tc32_kernel<T, GROUPED>, dim3((unsigned)grid), dim3(T32_THREADS), (size_t)Tc32Smem::TOTAL, st, a));
     b200_count_launch();
     return B200_OK;
 }
@@ -314,13 +337,13 @@ int b200_mmq_tc32(int type, const void * W, const float * X, int64_t x_col_strid
     if (((uintptr_t)W | (uintptr_t)X | (uintptr_t)workspace) & 15 || (x_col_stride & 3)) { b200_set_error("mul_mat_q: pointers must be 16-byte aligned"); return B200_ERR_INVALID; }
     if (k_valid <= 0 || k_valid > k || k_valid % 8 != 0) { b200_set_error("mul_mat_q: k_valid must be a positive multiple of 8, at most k"); return B200_ERR_INVALID; }
     const Tc32Geom g = tc32_geom(k, ncols);
-    Tc32Args a;
+    Tc32Args a = {};
     a.W = (const uint8_t *)W; a.ws = (const uint8_t *)workspace; a.dst = dst; a.m = m; a.k = k; a.ncols = ncols; a.ldd = ldd;
     a.rb = (k / 32) * type_block_bytes(type); a.nt = g.nt; a.ns = (int32_t)g.ns;
     a.n_tiles = (int32_t)(((m + T32_TM - 1) / T32_TM) * g.nt);
     a.prof = b200_mmq_prof_buf();
     dim3 qgrid((unsigned)(k / 256), (unsigned)(g.nt * 16));
-    B200_CUDA(b200_launch_pdl(quantize_mmq32_kernel, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k_valid, (uint8_t *)workspace, g));
+    B200_CUDA(b200_launch_pdl(quantize_mmq32_kernel<false>, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k_valid, (uint8_t *)workspace, g, MmidMap{}));
     b200_count_launch();
     int rc = B200_ERR_UNSUPPORTED;
     switch (type) {
@@ -329,5 +352,28 @@ int b200_mmq_tc32(int type, const void * W, const float * X, int64_t x_col_strid
         case B200_TYPE_Q8_0: rc = tc32_launch<B200_TYPE_Q8_0>(a, st); break;
     }
     if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc32", type, m, k, ncols, a.n_tiles, st);
+    return rc;
+}
+
+// grouped MUL_MAT_ID (mmid_route.cu): B f32 activations gathered through map, W the first expert, n_ct the upper bound of column tiles;
+// `image` (16-byte aligned) holds b200_mmq_tc32_workspace(k, 128 * n_ct) bytes
+int b200_mmq_tc32_grouped(int type, const void * W, const float * B, float * dst, int64_t m, int64_t k, int64_t n_ct, const MmidMap & map, void * image, cudaStream_t st) {
+    const Tc32Geom g = tc32_geom(k, n_ct * T32_TN);
+    Tc32Args a = {};
+    a.W = (const uint8_t *)W; a.ws = (const uint8_t *)image; a.dst = dst; a.m = m; a.k = k; a.ncols = n_ct * T32_TN;
+    a.rb = (k / 32) * type_block_bytes(type); a.nt = g.nt; a.ns = (int32_t)g.ns;
+    a.n_mtiles = (int32_t)((m + T32_TM - 1) / T32_TM); a.n_tiles = (int32_t)(a.n_mtiles * n_ct);
+    a.prof = b200_mmq_prof_buf();
+    a.map = map;
+    dim3 qgrid((unsigned)(k / 256), (unsigned)(n_ct * 16));
+    B200_CUDA(b200_launch_pdl(quantize_mmq32_kernel<true>, qgrid, dim3(256), 0, st, B, (int64_t)0, a.ncols, k, (uint8_t *)image, g, map));
+    b200_count_launch();
+    int rc = B200_ERR_UNSUPPORTED;
+    switch (type) {
+        case B200_TYPE_Q4_0: rc = tc32_launch<B200_TYPE_Q4_0, true>(a, st); break;
+        case B200_TYPE_Q5_0: rc = tc32_launch<B200_TYPE_Q5_0, true>(a, st); break;
+        case B200_TYPE_Q8_0: rc = tc32_launch<B200_TYPE_Q8_0, true>(a, st); break;
+    }
+    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc32 grouped", type, m, k, a.ncols, a.n_tiles, st);
     return rc;
 }
