@@ -1000,6 +1000,7 @@ uint64_t topology_key(const b200_node * nodes, int n, int flags) {
     for (int i = 0; i < n; i++) {
         const b200_node & nd = nodes[i];
         h = mix(h, (uint64_t)nd.op | ((uint64_t)nd.n_src << 32));
+        h = mix(h, (uint64_t)(uint32_t)nd.dst.flags);   // an OUTPUT result is materialised where an unflagged one may be fused away
         h = mix(h, (uint64_t)(uintptr_t)nd.dst.data); h = mix(h, (uint64_t)nd.dst.ne[0] ^ ((uint64_t)nd.dst.ne[1] << 24) ^ ((uint64_t)nd.dst.ne[2] << 48)); h = mix(h, (uint64_t)nd.dst.nb[1]);
         for (int s = 0; s < nd.n_src && s < B200_MAX_SRC; s++) {
             const b200_tensor & t = nd.src[s];

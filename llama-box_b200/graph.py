@@ -12,6 +12,7 @@ F32, F16, Q4_0, Q5_0, Q8_0, Q4_K, Q5_K, Q6_K, I32, I64 = 0, 1, 2, 6, 8, 12, 13, 
 Q4_1, Q5_1, Q2_K, Q3_K, IQ4_NL, IQ4_XS, MXFP4 = 3, 7, 10, 11, 20, 23, 39      # the wide path's formats (b200_ops.h)
 OP_NONE, OP_MUL_MAT, OP_RMS_NORM, OP_MUL, OP_ADD, OP_ROPE, OP_SET_ROWS, OP_FLASH_ATTN_EXT, OP_GLU_SWIGLU, OP_GET_ROWS, OP_CPY, OP_MUL_MAT_ID, OP_SOFT_MAX, OP_ARGSORT, OP_SUM_ROWS, OP_DIV, OP_CONT, OP_SCALE, OP_UNARY = range(19)
 EXEC_CUDA_GRAPHS, EXEC_FUSION, EXEC_MEGAKERNEL, EXEC_MEGA_MMV = 1, 2, 4, 8
+FLAG_OUTPUT = 2                     # B200_TENSOR_FLAG_OUTPUT (== GGML_TENSOR_FLAG_OUTPUT): the caller reads this tensor
 MAX_SRC = 6
 ELEM_SIZE = {F32: 4, F16: 2, I32: 4, I64: 8}
 
@@ -55,6 +56,7 @@ class T:
             nb = [ELEM_SIZE.get(type_, ops.lib.b200_block_bytes(type_) or 1), row_size(type_, ne[0]), 0, 0]
             nb[2] = nb[1] * ne[1]; nb[3] = nb[2] * ne[2]
         self.ptr, self.type, self.ne, self.nb = int(ptr), type_, ne, list(nb)
+        self.flags = 0
         if tid is None:
             tid = _next_id[0]; _next_id[0] += 1
         self.id = tid
@@ -67,7 +69,7 @@ class T:
         return T(self.ptr, self.type, ne)
 
     def fill(self, ct):
-        ct.id, ct.data, ct.type, ct.flags = self.id, self.ptr, self.type, 0
+        ct.id, ct.data, ct.type, ct.flags = self.id, self.ptr, self.type, self.flags
         for i in range(4):
             ct.ne[i] = self.ne[i]; ct.nb[i] = self.nb[i]
 

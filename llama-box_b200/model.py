@@ -87,6 +87,8 @@ class Weights:
 
 
 class SyntheticLlama:
+    device = "cuda"                 # where the io buffers of build() live
+
     def __init__(self, cfg, ftype="Q4_K_M", n_ctx=4096, kv_type=G.F16, seed=1234, host_weights=None, n_layer=None,
                  layer_range=None, first=True, last=True, n_seq=1):
         c = dict(CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
@@ -143,21 +145,26 @@ class SyntheticLlama:
     def _buf(self, name, shape, dtype=torch.float32):
         key = (name, tuple(shape), dtype)
         if key not in self.bufs:
-            self.bufs[key] = torch.zeros(shape, dtype=dtype, device="cuda")
+            self.bufs[key] = torch.zeros(shape, dtype=dtype, device=self.device)
         return self.bufs[key]
 
-    def build(self, n_tok, n_kv, want_all_logits=False, seq=0, skip_attention=False):
+    def build(self, n_tok, n_kv, want_all_logits=False, seq=0, skip_attention=False, n_out=1, place=None):
         """node list for one ubatch of n_tok tokens attending to n_kv cache positions (n_kv % 256 == 0 with -fa).
         skip_attention (bench roofline leg only): leave out ROPE / SET_ROWS / FLASH_ATTN_EXT and feed the Q projection
         straight into wo, so that the list holds exactly the step's matvec launches with their in-situ prologues
         (rms_norm + quantise inside the kernel, residual epilogues, lm_head) and nothing else.
         Inputs (device buffers the caller fills): tokens i32[n_tok], pos i32[n_tok], kv_idx i64[n_tok],
-        mask f32[n_kv, pad64(n_tok)] (cast to f16 by a CPY node like llama-graph.cpp:1424), out_ids i32[n_out]."""
+        mask f32[n_kv, pad64(n_tok)] (cast to f16 by a CPY node like llama-graph.cpp:1424), out_ids i32[n_out]
+        (n_out rows of logits unless want_all_logits).
+        place: optional placement hook, called as place(nl, fixed) before the list is built.  It may move every
+        intermediate (the dst of a compute node other than SET_ROWS, and the views of it) to addresses of its choosing,
+        the way a graph allocator recycles buffers; `fixed` are the results the caller reads from io (hidden_out,
+        logits) and must stay put.  Without it every intermediate has a buffer of its own."""
         c = self.c
         E, H, HK, D, FF, V = c["n_embd"], c["n_head"], c["n_head_kv"], c["head_dim"], c["n_ff"], c["n_vocab"]
         nl = G.NodeList()
         npad = (n_tok + 63) // 64 * 64
-        n_out = n_tok if want_all_logits else 1
+        n_out = n_tok if want_all_logits else n_out
         io = dict(tokens=self._buf("tokens", [n_tok], torch.int32), pos=self._buf("pos", [n_tok], torch.int32), kv_idx=self._buf("kv_idx", [n_tok], torch.int64),
                   mask=self._buf("mask", [npad, n_kv]), out_ids=self._buf("out_ids", [n_out], torch.int32), logits=self._buf("logits", [n_out, V]),
                   hidden_in=self._buf("hidden_in", [n_tok, E]), hidden_out=self._buf("hidden_out", [n_tok, E]))
@@ -172,8 +179,9 @@ class SyntheticLlama:
             inpL = nl.add(G.OP_GET_ROWS, tT(f("inp_embd", [E, n_tok]), G.F32, [E, n_tok]), [tT(self.tok_embd, G.F32, [E, V]), tT(io["tokens"], G.I32, [n_tok])])
         else:
             inpL = tT(io["hidden_in"], G.F32, [E, n_tok])          # handed over by the previous pipeline stage
-        rope_params = [0, D, c["rope_mode"], 0, 8192, G.f32_bits(c["rope_base"]), G.f32_bits(1.0), G.f32_bits(0.0), G.f32_bits(1.0), G.f32_bits(32.0), G.f32_bits(1.0)]
-        ff_t = tT(self.rope_ff, G.F32, [D // 2]) if self.rope_ff is not None else None
+        n_dims = c.get("rope_n_dims", D)                        # partial rotary: the first n_dims of each head
+        rope_params = [0, n_dims, c["rope_mode"], 0, 8192, G.f32_bits(c["rope_base"]), G.f32_bits(1.0), G.f32_bits(0.0), G.f32_bits(1.0), G.f32_bits(32.0), G.f32_bits(1.0)]
+        ff_t = tT(self.rope_ff, G.F32, [self.rope_ff.numel()]) if self.rope_ff is not None else None
         kvrow = G.row_size(self.kv_type, HK * D); kvhead = G.row_size(self.kv_type, D)
         for il, ly in enumerate(self.layers):
             last = self.last and il == len(self.layers) - 1
@@ -233,9 +241,15 @@ class SyntheticLlama:
             l_out = tT(io["hidden_out"], G.F32, [E, nt]) if final_stage_out else tT(f(f"l_out{il % 2}", [E, nt]), G.F32, [E, nt])
             inpL = nl.add(G.OP_ADD, l_out, [dn, ffn_inp])
         if not self.last:
+            if place is not None:
+                place(nl, [inpL])
             return nl.build(), io
         nt = n_out
         t1 = nl.add(G.OP_RMS_NORM, tT(f("onorm", [E, nt]), G.F32, [E, nt]), [inpL], [G.f32_bits(c["eps"])])
         cur = nl.add(G.OP_MUL, tT(f("onormw", [E, nt]), G.F32, [E, nt]), [t1, tT(self.output_norm, G.F32, [E])])
-        nl.add(G.OP_MUL_MAT, tT(io["logits"], G.F32, [V, nt]), [self.output.t, cur])
+        logits = tT(io["logits"], G.F32, [V, nt])
+        logits.flags = G.FLAG_OUTPUT                           # libllama flags t_logits (llama-context.cpp graph outputs)
+        nl.add(G.OP_MUL_MAT, logits, [self.output.t, cur])
+        if place is not None:
+            place(nl, [logits])
         return nl.build(), io

@@ -52,43 +52,51 @@ class OracleLlama:
     def rope(self, x, pos, nh):
         c = self.c; D = c["head_dim"]; n = x.shape[0]
         y = np.zeros_like(x)
-        oracle().orc_rope(ptr(x), ptr(y), ptr(pos), ptr(self.ff), D, nh, n, D, c["rope_mode"], 8192, c["rope_base"], 1.0, 0.0, 1.0, 32.0, 1.0)
+        oracle().orc_rope(ptr(x), ptr(y), ptr(pos), ptr(self.ff), D, nh, n, c.get("rope_n_dims", D), c["rope_mode"], 8192, c["rope_base"], 1.0, 0.0, 1.0, 32.0, 1.0)
         return y
 
     def forward(self, tokens, pos, kv_idx, n_kv, mask16, trace=None):
         """tokens i32[n], pos i32[n], kv_idx i64[n], mask16 uint16 [npad, n_kv] -> logits of the last token [V]"""
+        x = np.ascontiguousarray(self.hw["token_embd"][tokens])
+        for il in range(self.c["n_layer"]):
+            x = self.layer(il, x, pos, kv_idx, n_kv, mask16, [len(tokens) - 1] if il == self.c["n_layer"] - 1 else None, trace)
+        return self.logits(x)[0]
+
+    def logits(self, x):
+        """output norm + output matrix of the rows x [n_out, n_embd] -> [n_out, V]"""
+        return self.mm("output", self.norm(x, self.hw["output_norm"]))
+
+    def layer(self, il, x, pos, kv_idx, n_kv, mask16, out_ids=None, trace=None):
+        """one layer on x [n, n_embd]: stores the new K / V rows in this layer's cache and returns the layer's output,
+        of the rows out_ids only if given (the last layer's output-row selection, llama-model.cpp:6054-6058)"""
         c = self.c
         H, HK, D = c["n_head"], c["n_head_kv"], c["head_dim"]
-        n = len(tokens)
-        x = np.ascontiguousarray(self.hw["token_embd"][tokens])
-        for il in range(c["n_layer"]):
-            cur = self.norm(x, self.hw[f"blk.{il}.attn_norm"])
-            q, k, v = self.mm(f"blk.{il}.attn_q", cur), self.mm(f"blk.{il}.attn_k", cur), self.mm(f"blk.{il}.attn_v", cur)
-            if c.get("qkv_bias"):
-                q = q + self.hw[f"blk.{il}.bq"]; k = k + self.hw[f"blk.{il}.bk"]; v = v + self.hw[f"blk.{il}.bv"]
-            q_pre = q
-            q = self.rope(np.ascontiguousarray(q), pos, H); k = self.rope(np.ascontiguousarray(k), pos, HK)
-            oracle().orc_set_rows(ptr(k), ptr(kv_idx), ptr(self.kc[il]), self.kv_type, HK * D, n, self.kvrow)
-            oracle().orc_set_rows(ptr(np.ascontiguousarray(v)), ptr(kv_idx), ptr(self.vc[il]), self.kv_type, HK * D, n, self.kvrow)
-            att = np.zeros((n, H * D), np.float32)
-            hb = row_bytes(self.kv_type, D)
-            oracle().orc_flash_attn_ext(ptr(q), H * D * 4, D * 4, ptr(self.kc[il]), self.kvrow, hb, ptr(self.vc[il]), self.kvrow, hb, ptr(mask16), ptr(att),
-                                        self.kv_type, D, D, H, HK, n, n_kv, 1.0 / math.sqrt(D), 0.0, 0.0)
-            o = self.mm(f"blk.{il}.attn_output", att)
-            if trace is not None and il == 0:
-                trace.update(normw0=cur, q=q_pre, qr=q, kr=k, v=v, att=att, wo=o)
-            if il == c["n_layer"] - 1:
-                o, x = o[-1:], x[-1:]
-            ffn_inp = o + x
-            cur = self.norm(ffn_inp, self.hw[f"blk.{il}.ffn_norm"])
-            up, gate = self.mm(f"blk.{il}.ffn_up", cur), self.mm(f"blk.{il}.ffn_gate", cur)
-            h = np.zeros_like(gate); oracle().orc_swiglu(ptr(gate), ptr(up), ptr(h), gate.size)
-            dn = self.mm(f"blk.{il}.ffn_down", h)
-            if trace is not None and il == 0:
-                trace.update(ffn_inp0=ffn_inp, fnormw=cur, up=up, gate=gate, h=h, down=dn)
-            x = dn + ffn_inp
-        cur = self.norm(x, self.hw["output_norm"])
-        return self.mm("output", cur)[0]
+        n = x.shape[0]
+        cur = self.norm(x, self.hw[f"blk.{il}.attn_norm"])
+        q, k, v = self.mm(f"blk.{il}.attn_q", cur), self.mm(f"blk.{il}.attn_k", cur), self.mm(f"blk.{il}.attn_v", cur)
+        if c.get("qkv_bias"):
+            q = q + self.hw[f"blk.{il}.bq"]; k = k + self.hw[f"blk.{il}.bk"]; v = v + self.hw[f"blk.{il}.bv"]
+        q_pre = q
+        q = self.rope(np.ascontiguousarray(q), pos, H); k = self.rope(np.ascontiguousarray(k), pos, HK)
+        oracle().orc_set_rows(ptr(k), ptr(kv_idx), ptr(self.kc[il]), self.kv_type, HK * D, n, self.kvrow)
+        oracle().orc_set_rows(ptr(np.ascontiguousarray(v)), ptr(kv_idx), ptr(self.vc[il]), self.kv_type, HK * D, n, self.kvrow)
+        att = np.zeros((n, H * D), np.float32)
+        hb = row_bytes(self.kv_type, D)
+        oracle().orc_flash_attn_ext(ptr(q), H * D * 4, D * 4, ptr(self.kc[il]), self.kvrow, hb, ptr(self.vc[il]), self.kvrow, hb, ptr(mask16), ptr(att),
+                                    self.kv_type, D, D, H, HK, n, n_kv, 1.0 / math.sqrt(D), 0.0, 0.0)
+        o = self.mm(f"blk.{il}.attn_output", att)
+        if trace is not None and il == 0:
+            trace.update(normw0=cur, q=q_pre, qr=q, kr=k, v=v, att=att, wo=o)
+        if out_ids is not None:
+            o, x = o[list(out_ids)], x[list(out_ids)]
+        ffn_inp = o + x
+        cur = self.norm(ffn_inp, self.hw[f"blk.{il}.ffn_norm"])
+        up, gate = self.mm(f"blk.{il}.ffn_up", cur), self.mm(f"blk.{il}.ffn_gate", cur)
+        h = np.zeros_like(gate); oracle().orc_swiglu(ptr(gate), ptr(up), ptr(h), gate.size)
+        dn = self.mm(f"blk.{il}.ffn_down", h)
+        if trace is not None and il == 0:
+            trace.update(ffn_inp0=ffn_inp, fnormw=cur, up=up, gate=gate, h=h, down=dn)
+        return dn + ffn_inp
 
 
 def causal_mask(n_tok, n_kv, pos0):
