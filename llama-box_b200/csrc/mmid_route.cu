@@ -10,15 +10,7 @@
 // Every output is folded by one CTA over its blocks in order from exact integer sums, so it is bit-identical to what b200_mul_mat_q gives
 // for the same expert matrix and the same activation column.  The launches are sized from the host's upper bound on the column tiles,
 // floor(N / 128) + min(n_expert, N) with N = n_tok * n_used; CTAs past the real count (in device memory) do nothing.
-#include "common.cuh"
-#include "mmid.cuh"
-
-#include <cstdlib>
-
-int64_t b200_mmq_tc_workspace(int64_t k, int64_t ncols);
-int64_t b200_mmq_tc32_workspace(int64_t k, int64_t ncols);
-int b200_mmq_tc_grouped(int type, const void * W, const float * B, float * dst, int64_t m, int64_t k, int64_t n_ct, const MmidMap & map, void * image, cudaStream_t st);
-int b200_mmq_tc32_grouped(int type, const void * W, const float * B, float * dst, int64_t m, int64_t k, int64_t n_ct, const MmidMap & map, void * image, cudaStream_t st);
+#include "mmq_tile.cuh"
 
 // When the grouped GEMM runs: at least MMID_MIN_TOK tokens (fewer — decode, speculative verify batches — stay on the matvec of mmvq_ext.cu,
 // one pass over an expert's weights per (token, slot)), and at least MMID_MIN_PAIRS (token, slot) pairs per expert on average.  A tile pass
@@ -48,21 +40,16 @@ RouteGeom route_geom(int type, int64_t k, int64_t n_expert, int64_t n_used, int6
     g.off_tiles = up256(g.off_cnt + 4 * n_expert);
     g.off_cols = up256(g.off_tiles + 4 * g.ub);
     g.off_image = up256(g.off_cols + 4 * 128 * g.ub);
-    g.total = g.off_image + (type_is_block32(type) ? b200_mmq_tc32_workspace(k, 128 * g.ub) : b200_mmq_tc_workspace(k, 128 * g.ub));
+    g.total = g.off_image + mmq_tile_workspace(type, k, 128 * g.ub);
     return g;
 }
 
 bool mmid_tc_ok(int type, int64_t m, int64_t k, int64_t n_expert, int64_t n_used, int64_t n_tok) {
-    static const bool off = getenv("B200_MMQ_DISABLE_TC") != nullptr;     // comparison arm: the matvec, as for the batched MUL_MAT
-    if (off || n_tok < MMID_MIN_TOK || m <= 0 || k <= 0 || n_expert <= 0 || n_expert > MMID_MAX_EXPERT || n_used <= 0 || n_used > n_expert) return false;
+    if (!mmq_tile_takes(type, m, k)) return false;
+    if (n_tok < MMID_MIN_TOK || n_expert <= 0 || n_expert > MMID_MAX_EXPERT || n_used <= 0 || n_used > n_expert) return false;
     if (n_tok * n_used > INT32_MAX / 2 || n_tok * n_used < MMID_MIN_PAIRS * n_expert) return false;
     const int64_t N = n_tok * n_used, ub = N / 128 + (n_expert < N ? n_expert : N);
-    if (ub * 16 > 65535 || ((m + 127) / 128) * ub > INT32_MAX) return false;          // quantiser grid.y, tile count
-    switch (type) {
-        case B200_TYPE_Q4_K: case B200_TYPE_Q5_K: case B200_TYPE_Q4_0: case B200_TYPE_Q5_0: case B200_TYPE_Q8_0: return k % 256 == 0;
-        case B200_TYPE_Q6_K: return k % 2048 == 0;
-        default: return false;
-    }
+    return ub * 16 <= 65535 && ((m + 127) / 128) * ub <= INT32_MAX;                    // quantiser grid.y, tile count
 }
 
 // one CTA of nw warps.  Warp w owns pairs [w * seg, (w + 1) * seg) of the list p = t * n_used + s.  Pass 1 counts each warp's pairs per
@@ -165,6 +152,6 @@ extern "C" int b200_mul_mat_id2(int type, const void * as, int64_t expert_stride
     B200_CUDA(b200_launch_pdl(mmid_route_kernel, dim3(1), dim3(32 * nw), smem, st, ids, ids_tok_stride, (int)n_expert, (int)n_used, n_tok,
                               (int32_t *)ws, (int32_t *)(ws + g.off_cnt), (int32_t *)(ws + g.off_tiles), (int32_t *)(ws + g.off_cols)));
     b200_count_launch();
-    return type_is_block32(type) ? b200_mmq_tc32_grouped(type, as, b, dst, m, k, g.ub, map, ws + g.off_image, st)
-                                 : b200_mmq_tc_grouped(type, as, b, dst, m, k, g.ub, map, ws + g.off_image, st);
+    const MmqJob job = { as, b, 0, k, dst, 0, m, k, 128 * g.ub, ws + g.off_image, &map };
+    return mmq_tile_run(type, job, st);
 }

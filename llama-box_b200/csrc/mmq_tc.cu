@@ -32,20 +32,13 @@
 // Shared memory (per CTA, ~150 KB): 2 A stages x 32 KB (128 rows x 128 k f16) + 2 B stages x 32 KB + the imin operands + scale rings.
 // Data movement: weights are read from HBM once per 128-token tile (L2 serves the other token tiles of the same rows, which
 // run on neighbouring CTAs), activations stream from L2.
-#include "common.cuh"
+#include "mmq_tile.cuh"
 #include "wgmma.cuh"
-#include "mmid.cuh"
 
 #include <cuda_fp16.h>
-#include <cstdio>
-#include <cstdlib>
 
-#define TC_TM 128
-#define TC_TN 128
-#define TC_THREADS 384
 #define TC_STAGE_A 32768
 #define TC_STAGE_B 32768
-#define TC_PANEL 2048             // one K-chunk (8 f16 = 16 bytes) of 128 rows
 
 // ---- workspace geometry (the B image) ------------------------------------------------------------------------------
 // per 128-token tile nt: Bq[nt][kq = k/64][chunk 0..7][n 0..127][8 f16]   (16 KB per 64-k quarter)
@@ -54,7 +47,7 @@
 struct TcGeom { int64_t nt, kq, nsb, off_bq, off_bm, off_d8, total; };
 static TcGeom tc_geom(int64_t k, int64_t ncols) {
     TcGeom g;
-    g.nt = (ncols + TC_TN - 1) / TC_TN; g.kq = k / 64; g.nsb = k / 256;
+    g.nt = (ncols + MMQ_TN - 1) / MMQ_TN; g.kq = k / 64; g.nsb = k / 256;
     g.off_bq = 0;
     g.off_bm = g.nt * g.kq * 16384;
     g.off_d8 = g.off_bm + g.nt * g.nsb * 4096;
@@ -65,31 +58,19 @@ static TcGeom tc_geom(int64_t k, int64_t ncols) {
 // ---- activation quantisation into the B image -------------------------------------------------------------------------
 // one warp per (token, super-block); exactly quantize_row_q8_K_ref: first index of the largest |x|, iscale = -127/max,
 // nearest-int (RNE), MIN(127, .), d = 1/iscale, bsums per 16
-// GATHER (grouped MUL_MAT_ID, mmid.cuh): column n of the image is the pair map.cols[n] of the activation x (zeros for padding); the blocks
+// GATHER (grouped MUL_MAT_ID): column n of the image is the pair map.cols[n] of the activation x (zeros for padding); the blocks
 // of column tiles past *map.ntt exit.  Each column's image is the one the dense instance writes for the same f32 column.
 template <bool GATHER>
-__global__ void __launch_bounds__(256) quantize_mmq_kernel(const float * __restrict__ x, int64_t x_col_stride, int64_t ncols, int64_t k,
+__global__ void __launch_bounds__(256) quantize_mmq_kernel(const float * __restrict__ x, int64_t x_col_stride, int64_t ncols, int64_t k_valid,
                                                           uint8_t * __restrict__ ws, TcGeom g, MmidMap map) {
     pdl_wait();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t sb = blockIdx.x;
     const int64_t n = (int64_t)blockIdx.y * 8 + warp;                // token (padded range: < nt * 128)
     const int64_t nt = n >> 7; const int nl = (int)(n & 127);
+    if constexpr (GATHER) { if (nt >= *map.ntt) return; }            // the whole block: blockIdx.y / 16 is its column tile
     float v[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    if constexpr (GATHER) {
-        if (nt >= *map.ntt) return;                                  // the whole block: blockIdx.y / 16 is its column tile
-        const int pr = map.cols[n], nu = map.n_used;
-        if (pr >= 0) {
-            const int t = pr / nu, s = pr % nu;
-            const float4 * p = (const float4 *)(x + (int64_t)t * map.b_tok_stride + (s % map.n_b1) * map.b_slot_stride + sb * 256 + lane * 8);
-            const float4 a = p[0], b = p[1];
-            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-        }
-    } else if (n < ncols) {
-        const float4 * p = (const float4 *)(x + n * x_col_stride + sb * 256 + lane * 8);
-        const float4 a = p[0], b = p[1];
-        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-    }
+    mmq_load_col8<GATHER>(v, x, x_col_stride, ncols, k_valid, map, n, sb * 256 + lane * 8);
     float am = 0.0f; int ai = 0;
 #pragma unroll
     for (int j = 0; j < 8; j++) { const float a = fabsf(v[j]); if (a > am) { am = a; ai = lane * 8 + j; } }
@@ -118,26 +99,19 @@ __global__ void __launch_bounds__(256) quantize_mmq_kernel(const float * __restr
     auto h2 = [](int a, int b) { return (uint32_t)__half_as_ushort(__int2half_rn(a)) | ((uint32_t)__half_as_ushort(__int2half_rn(b)) << 16); };
     uint4 pk; pk.x = h2(q[0], q[2]); pk.y = h2(q[1], q[3]); pk.z = h2(q[4], q[6]); pk.w = h2(q[5], q[7]);
     const int64_t kq = sb * 4 + (lane >> 3); const int c = lane & 7;
-    *(uint4 *)(ws + g.off_bq + ((nt * g.kq + kq) * 8 + c) * TC_PANEL + nl * 16) = pk;
+    *(uint4 *)(ws + g.off_bq + ((nt * g.kq + kq) * 8 + c) * MMQ_PANEL + nl * 16) = pk;
     s += __shfl_xor_sync(0xffffffffu, s, 1);                          // bsum of 16 elements (|.| <= 2032: exact in f16)
     if ((lane & 1) == 0) {
         const int grp = lane >> 1;
-        *(__half *)(ws + g.off_bm + ((nt * g.nsb + sb) * 2 + (grp >> 3)) * TC_PANEL + nl * 16 + (grp & 7) * 2) = __int2half_rn(s);
+        *(__half *)(ws + g.off_bm + ((nt * g.nsb + sb) * 2 + (grp >> 3)) * MMQ_PANEL + nl * 16 + (grp & 7) * 2) = __int2half_rn(s);
     }
     if (lane == 0) *(float *)(ws + g.off_d8 + ((nt * g.nsb + sb) * 128 + nl) * 4) = d;
     pdl_trigger();
 }
 
-struct TcArgs {
-    const uint8_t * W;          // weights, `type` rows (Q6_K: repacked rows, see repack.cu)
-    const uint8_t * ws;         // B image (quantize_mmq_kernel)
-    float *         dst;        // [ncols][ldd] f32
-    int64_t m, k, ncols, ldd, rb;
+struct TcArgs : MmqTileArgs {
     TcGeom g;
-    int32_t nsb, n_mtiles, n_tiles, type;
     uint32_t lbo, sbo;          // descriptor strides (bytes): K-chunk stride / 8-row-group stride
-    unsigned long long * prof;  // bring-up: per-role cycle counters of CTA 0 (B200_MMQ_PROF), normally null
-    MmidMap map;                // GROUPED only: W is the first expert's matrix, columns are (token, slot) pairs
 };
 // ---- per-type pipeline geometry: K-stages per super-block, whether the mins MMA runs, activation bytes per stage -------
 // (the transform threads read each row's packed blocks straight from global memory, so no weight bytes live in shared memory;
@@ -170,10 +144,10 @@ __device__ __forceinline__ void k4_unpack(uint32_t y, uint32_t z, uint32_t w, ui
     mn47 = ((w >> 4) & 0x0f0f0f0fu) | (((z >> 6) & 0x03030303u) << 4);
 }
 
-// GROUPED (MUL_MAT_ID, mmid.cuh): column tile ct multiplies expert map.tile_expert[ct]; the tile count comes from the device (*map.ntt)
+// GROUPED (MUL_MAT_ID): column tile ct multiplies expert map.tile_expert[ct]; the tile count comes from the device (*map.ntt)
 // and the epilogue scatters column j to its pair's output row (padding columns are not stored).  Everything else is the dense kernel.
 template <int T, bool GROUPED>
-__global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_constant__ TcArgs args) {
+__global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc_kernel(const __grid_constant__ TcArgs args) {
     using TT = TcType<T>;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t * bars = (uint64_t *)(smem + TcSmem::BAR);
@@ -187,10 +161,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
     __syncthreads();
     pdl_wait();
 
-    const int nsb = args.nsb;
-    const auto NT = [&]() { if constexpr (GROUPED) return *args.map.ntt; else return args.g.nt; }();     // column tiles (grouped: 32-bit tile arithmetic)
+    const int nsb = args.nks;
+    const auto NT = mmq_col_tiles<GROUPED>(args);
     auto n_tiles = [&]() { return GROUPED ? args.n_mtiles * (int)NT : args.n_tiles; };      // dense: read from the parameters at each use
-    unsigned long long w0 = 0, w1 = 0, w2 = 0;                       // profile: cycles in this role's kinds of waits
+    unsigned long long w0 = 0, w1 = 0;                               // profile: cycles in this role's kinds of waits
     const bool prof = args.prof != nullptr && blockIdx.x == 0;
     unsigned long long * pw0 = prof ? &w0 : nullptr, * pw1 = prof ? &w1 : nullptr;
     const long long t_start = clock64();
@@ -223,10 +197,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
         uint32_t it = 0, sbc = 0;
         uint4 nxt[NW]; uint16_t nxt_d = 0;
         auto fetch = [&](int tile, int sb) {
-            const int64_t m0 = (int64_t)(tile / NT) * TC_TM;
-            int64_t r = m0 + t; if (r >= args.m) r = args.m - 1;             // rows past the end: any valid row (their results are never stored)
-            const uint8_t * row = args.W + r * args.rb;
-            if constexpr (GROUPED) row += (int64_t)args.map.tile_expert[tile - (m0 / TC_TM) * NT] * args.map.expert_stride;   // column tile = tile % NT
+            const int64_t mt = tile / NT;
+            const uint8_t * row = mmq_weight_row<GROUPED>(args, mt, tile - mt * NT, t);
             if (T == B200_TYPE_Q6_K) {
                 const uint4 * ql = (const uint4 *)(row + (int64_t)sb * 128), * qh = (const uint4 *)(row + nb * 128 + (int64_t)sb * 64);
 #pragma unroll
@@ -293,8 +265,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                                     plo[2 * u] = hfma2_u(l0, m_lo, c_lo); plo[2 * u + 1] = hfma2_u(l1, m_lo, c_lo);     // exact: sc * q
                                     phi[2 * u] = hfma2_u(h0, m_hi, c_hi); phi[2 * u + 1] = hfma2_u(h1, m_hi, c_hi);
                                 }
-                                *(uint4 *)(As + (gg * 8 + i) * TC_PANEL) = lo;
-                                *(uint4 *)(As + (gg * 8 + 4 + i) * TC_PANEL) = hi;
+                                *(uint4 *)(As + (gg * 8 + i) * MMQ_PANEL) = lo;
+                                *(uint4 *)(As + (gg * 8 + 4 + i) * MMQ_PANEL) = hi;
                             }
                         }
                         if (s == 0) {
@@ -303,7 +275,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                             uint4 m0, m1;
                             m0.x = h2_of_int(mn03 & 63); m0.y = h2_of_int((mn03 >> 8) & 63); m0.z = h2_of_int((mn03 >> 16) & 63); m0.w = h2_of_int((mn03 >> 24) & 63);
                             m1.x = h2_of_int(mn47 & 63); m1.y = h2_of_int((mn47 >> 8) & 63); m1.z = h2_of_int((mn47 >> 16) & 63); m1.w = h2_of_int((mn47 >> 24) & 63);
-                            *(uint4 *)Am = m0; *(uint4 *)(Am + TC_PANEL) = m1;
+                            *(uint4 *)Am = m0; *(uint4 *)(Am + MMQ_PANEL) = m1;
                             rscale[t] = make_float2(h2f((uint16_t)(hdr.x & 0xffff)), h2f((uint16_t)(hdr.x >> 16)));
                         }
                         fence_async_smem();                               // generic-proxy writes -> visible to the tensor core (async proxy)
@@ -344,8 +316,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                                     pe[2 * u] = hmul2_u(x0, m_e); pe[2 * u + 1] = hmul2_u(x1, m_e);                  // even scale part: exact (even integers <= 4096)
                                     po[2 * u] = hmul2_u(x0, m_o); po[2 * u + 1] = hmul2_u(x1, m_o);
                                 }
-                                *(uint4 *)(As + (tt * 4 + i) * TC_PANEL) = ev;
-                                *(uint4 *)(As + (8 + tt * 4 + i) * TC_PANEL) = od;
+                                *(uint4 *)(As + (tt * 4 + i) * MMQ_PANEL) = ev;
+                                *(uint4 *)(As + (8 + tt * 4 + i) * MMQ_PANEL) = od;
                             }
                         }
                         if (s == 0) rscale[t] = make_float2(h2f(cur_d), 0.0f);
@@ -379,7 +351,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
                         const uint32_t bj = TT::STAGES == 2 ? j : (j & 3);        // Q6_K: the even and the odd-scale pass read the same 64-k panel
-                        wg_mma_ss(frag, wg_desc(a0 + j * 2 * TC_PANEL, args.lbo, args.sbo), wg_desc(b0 + bj * 2 * TC_PANEL, args.lbo, args.sbo), (s | j) ? 1u : 0u);
+                        wg_mma_ss(frag, wg_desc(a0 + j * 2 * MMQ_PANEL, args.lbo, args.sbo), wg_desc(b0 + bj * 2 * MMQ_PANEL, args.lbo, args.sbo), (s | j) ? 1u : 0u);
                     }
                     wg_commit();
                     wg_wait0();
@@ -418,117 +390,36 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mmq_tc_kernel(const __grid_cons
                     }
                 }
             }
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int64_t row = mt * TC_TM + ra + 8 * h;
-                if (row >= args.m) continue;
-#pragma unroll
-                for (int j = 0; j < 16; j++) {
-#pragma unroll
-                    for (int e = 0; e < 2; e++) {
-                        const int64_t n = nt * TC_TN + 8 * j + c0 + e;
-                        if constexpr (GROUPED) {
-                            const int pr = args.map.cols[n], nu = args.map.n_used;
-                            if (pr >= 0) args.dst[(pr / nu) * args.map.dst_tok_stride + (pr % nu) * args.map.dst_slot_stride + row] = acc[4 * j + 2 * h + e];
-                        } else if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
-                    }
-                }
-            }
+            mmq_store_tile<GROUPED>(args, acc, mt, nt, ra, c0);
         }
     }
 
-    if (prof && lane == 0) {                                           // [warp][total, wait0, wait1, wait2]
-        unsigned long long * o = args.prof + warp * 4;
-        o[0] = (unsigned long long)(clock64() - t_start); o[1] = w0; o[2] = w1; o[3] = w2;
-    }
+    if (prof && lane == 0) mmq_prof_store(args, warp, t_start, w0, w1);
     pdl_trigger();
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
-unsigned long long * b200_mmq_prof_buf();
-void b200_mmq_prof_report(const char * kernel, int type, int64_t m, int64_t k, int64_t ncols, int n_tiles, cudaStream_t st);
-
-bool b200_mmq_tc_supported(int type, int64_t m, int64_t k, int64_t ncols) {
-    static const bool off = getenv("B200_MMQ_DISABLE_TC") != nullptr;     // debugging: stream column groups through the matvec kernel instead (still the GPU)
-    if (off || m <= 0 || ncols < 9) return false;
-    if (type == B200_TYPE_Q4_K || type == B200_TYPE_Q5_K) return k > 0 && k % 256 == 0;
-    if (type == B200_TYPE_Q6_K) return k > 0 && k % 2048 == 0;
-    return false;
-}
 int64_t b200_mmq_tc_workspace(int64_t k, int64_t ncols) { return tc_geom(k, ncols).total; }
 
-// grouped: a.n_tiles is the host's upper bound (the kernel reads the real count)
-template <int T, bool GROUPED = false> static int tc_launch(const TcArgs & a, cudaStream_t st) {
-    static bool attr[64] = { false };
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(mmq_tc_kernel<T, GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem::TOTAL)); attr[dev & 63] = true; }
-    int grid = a.n_tiles < b200_sm_count() ? a.n_tiles : b200_sm_count();
-    B200_CUDA(b200_launch_pdl(mmq_tc_kernel<T, GROUPED>, dim3((unsigned)grid), dim3(TC_THREADS), (size_t)TcSmem::TOTAL, st, a));
-    b200_count_launch();
-    return B200_OK;
-}
-
-int b200_mmq_tc(int type, const void * W, const float * X, int64_t x_col_stride, float * dst, int64_t ldd, int64_t m, int64_t k, int64_t ncols, void * workspace, void * stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (((uintptr_t)W | (uintptr_t)X | (uintptr_t)workspace) & 15 || (x_col_stride & 3)) { b200_set_error("mul_mat_q: pointers must be 16-byte aligned"); return B200_ERR_INVALID; }
-    TcArgs a = {};
-    a.W = (const uint8_t *)W; a.ws = (const uint8_t *)workspace; a.dst = dst; a.m = m; a.k = k; a.ncols = ncols; a.ldd = ldd;
-    a.rb = (k / 256) * type_block_bytes(type);
-    a.g = tc_geom(k, ncols);
-    a.lbo = (uint32_t)TC_PANEL; a.sbo = 128u;
-    a.prof = b200_mmq_prof_buf();
-    a.nsb = (int32_t)(k / 256); a.n_mtiles = (int32_t)((m + TC_TM - 1) / TC_TM); a.n_tiles = (int32_t)(a.n_mtiles * a.g.nt); a.type = type;
-    dim3 qgrid((unsigned)a.nsb, (unsigned)(a.g.nt * 16));
-    B200_CUDA(b200_launch_pdl(quantize_mmq_kernel<false>, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k, (uint8_t *)workspace, a.g, MmidMap{}));
-    b200_count_launch();
-    int rc = B200_ERR_UNSUPPORTED;
+template <bool GROUPED> static int tc_launch(int type, const TcArgs & a, cudaStream_t st) {
     switch (type) {
-        case B200_TYPE_Q4_K: rc = tc_launch<B200_TYPE_Q4_K>(a, st); break;
-        case B200_TYPE_Q5_K: rc = tc_launch<B200_TYPE_Q5_K>(a, st); break;
-        case B200_TYPE_Q6_K: rc = tc_launch<B200_TYPE_Q6_K>(a, st); break;
+        case B200_TYPE_Q4_K: return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q4_K, GROUPED>, TcSmem::TOTAL>(a, st);
+        case B200_TYPE_Q5_K: return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q5_K, GROUPED>, TcSmem::TOTAL>(a, st);
+        case B200_TYPE_Q6_K: return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q6_K, GROUPED>, TcSmem::TOTAL>(a, st);
     }
-    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc", type, m, k, ncols, a.n_tiles, st);
-    return rc;
+    return B200_ERR_UNSUPPORTED;
 }
 
-// grouped MUL_MAT_ID (mmid_route.cu): B f32 activations gathered through map, W the first expert, n_ct the upper bound of column tiles;
-// `image` (16-byte aligned) holds b200_mmq_tc_workspace(k, 128 * n_ct) bytes
-int b200_mmq_tc_grouped(int type, const void * W, const float * B, float * dst, int64_t m, int64_t k, int64_t n_ct, const MmidMap & map, void * image, cudaStream_t st) {
+int b200_mmq_tc(int type, const MmqJob & j, cudaStream_t st) {
     TcArgs a = {};
-    a.W = (const uint8_t *)W; a.ws = (const uint8_t *)image; a.dst = dst; a.m = m; a.k = k; a.ncols = n_ct * TC_TN;
-    a.rb = (k / 256) * type_block_bytes(type);
-    a.g = tc_geom(k, a.ncols);
-    a.lbo = (uint32_t)TC_PANEL; a.sbo = 128u;
-    a.prof = b200_mmq_prof_buf();
-    a.nsb = (int32_t)(k / 256); a.n_mtiles = (int32_t)((m + TC_TM - 1) / TC_TM); a.n_tiles = (int32_t)(a.n_mtiles * n_ct); a.type = type;
-    a.map = map;
-    dim3 qgrid((unsigned)a.nsb, (unsigned)(n_ct * 16));
-    B200_CUDA(b200_launch_pdl(quantize_mmq_kernel<true>, qgrid, dim3(256), 0, st, B, (int64_t)0, a.ncols, k, (uint8_t *)image, a.g, map));
+    mmq_tile_fill(a, j, (j.k / 256) * type_block_bytes(type));
+    a.g = tc_geom(j.k, j.ncols);
+    a.nks = (int32_t)(j.k / 256);
+    a.lbo = (uint32_t)MMQ_PANEL; a.sbo = 128u;
+    B200_CUDA(b200_launch_pdl(j.map ? quantize_mmq_kernel<true> : quantize_mmq_kernel<false>, dim3((unsigned)a.nks, (unsigned)(a.nt * 16)), dim3(256), 0, st,
+                              j.X, j.x_col_stride, j.ncols, j.k_valid, (uint8_t *)j.workspace, a.g, a.map));
     b200_count_launch();
-    int rc = B200_ERR_UNSUPPORTED;
-    switch (type) {
-        case B200_TYPE_Q4_K: rc = tc_launch<B200_TYPE_Q4_K, true>(a, st); break;
-        case B200_TYPE_Q5_K: rc = tc_launch<B200_TYPE_Q5_K, true>(a, st); break;
-        case B200_TYPE_Q6_K: rc = tc_launch<B200_TYPE_Q6_K, true>(a, st); break;
-    }
-    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc grouped", type, m, k, a.ncols, a.n_tiles, st);
+    const int rc = j.map ? tc_launch<true>(type, a, st) : tc_launch<false>(type, a, st);
+    if (a.prof && rc == B200_OK) mmq_prof_report(j.map ? "mmq_tc grouped" : "mmq_tc", type, a, st);
     return rc;
-}
-
-// B200_MMQ_PROF=1: per-role wait cycles of CTA 0 of the tile kernels (this file and mmq_tc32.cu, which share the warp roles),
-// printed after each launch (bring-up only)
-unsigned long long * b200_mmq_prof_buf() {
-    static unsigned long long * prof_buf = nullptr;
-    static const bool want_prof = getenv("B200_MMQ_PROF") != nullptr;
-    if (want_prof && !prof_buf) { cudaMalloc((void **)&prof_buf, 16 * 4 * 8); }
-    return want_prof ? prof_buf : nullptr;
-}
-void b200_mmq_prof_report(const char * kernel, int type, int64_t m, int64_t k, int64_t ncols, int n_tiles, cudaStream_t st) {
-    unsigned long long h[16 * 4];
-    cudaStreamSynchronize(st); cudaMemcpy(h, b200_mmq_prof_buf(), sizeof(h), cudaMemcpyDeviceToHost);
-    const char * role[12] = { "mma", "mma", "mma", "mma", "mma", "mma", "mma", "mma", "xform", "xform", "xform", "xform" };
-    fprintf(stderr, "%s prof (CTA 0, cycles): type %d m %lld k %lld n %lld tiles %d\n", kernel, type, (long long)m, (long long)k, (long long)ncols, n_tiles);
-    for (int w = 0; w < 12; w += (w < 8 ? 4 : 2))
-        fprintf(stderr, "  warp %2d %-8s total %9llu  wait0 %9llu  wait1 %9llu  wait2 %9llu\n", w, role[w], h[w * 4], h[w * 4 + 1], h[w * 4 + 2], h[w * 4 + 3]);
-    fprintf(stderr, "  (mma: wait0 = b_full, wait1 = a_full | xform: wait1 = ab_empty)\n");
 }

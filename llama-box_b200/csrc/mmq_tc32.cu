@@ -29,24 +29,13 @@
 //     warps 8-11       transform: thread t owns weight row t of the tile, reads its packed blocks one stage ahead from global
 //                      memory into registers; thread 0 also issues the activation panel of each stage (cp.async.bulk)
 // A stage is 128 k (4 blocks): A 16 KB (int8 core matrices) + B 16 KB + d_x 2 KB + d_w 2 KB; 4 stages, ~144 KB of shared memory.
-#include "common.cuh"
+#include "mmq_tile.cuh"
 #include "wgmma.cuh"
-#include "mmid.cuh"
 
-#include <cstdlib>
-
-#define T32_TM 128
-#define T32_TN 128
-#define T32_THREADS 384
 #define T32_KS 128                  // k per stage
 #define T32_NSTAGE 4
-#define T32_PANEL 2048              // one K-chunk (16 int8 = 16 bytes) of 128 rows
-#define T32_STAGE_A (8 * T32_PANEL)
-#define T32_STAGE_B (8 * T32_PANEL + 4 * 512)      // the panel + d_x of its 4 blocks
-
-// B200_MMQ_PROF (mmq_tc.cu)
-unsigned long long * b200_mmq_prof_buf();
-void b200_mmq_prof_report(const char * kernel, int type, int64_t m, int64_t k, int64_t ncols, int n_tiles, cudaStream_t st);
+#define T32_STAGE_A (8 * MMQ_PANEL)
+#define T32_STAGE_B (8 * MMQ_PANEL + 4 * 512)      // the panel + d_x of its 4 blocks
 
 // ---- workspace geometry (the activation image) --------------------------------------------------------------------------
 // per 128-token tile nt and 128-k stage ks, contiguous so that one stage is one run of bytes:
@@ -55,7 +44,7 @@ void b200_mmq_prof_report(const char * kernel, int type, int64_t m, int64_t k, i
 struct Tc32Geom { int64_t nt, ns, total; };
 static Tc32Geom tc32_geom(int64_t k, int64_t ncols) {
     Tc32Geom g;
-    g.nt = (ncols + T32_TN - 1) / T32_TN; g.ns = k / T32_KS;
+    g.nt = (ncols + MMQ_TN - 1) / MMQ_TN; g.ns = k / T32_KS;
     g.total = g.nt * g.ns * T32_STAGE_B;
     return g;
 }
@@ -63,7 +52,7 @@ static Tc32Geom tc32_geom(int64_t k, int64_t ncols) {
 // ---- activation quantisation into the image ------------------------------------------------------------------------------
 // one warp per (token, 256 elements), 4 lanes per q8_0 block: the arithmetic of warp_quant_q80 (actquant.cuh).  Elements from
 // k_valid up (padded weight rows) and tokens from ncols up are zeros with d = 0.
-// GATHER (grouped MUL_MAT_ID, mmid.cuh): column n of the image is the pair map.cols[n] of x (zeros for padding); the blocks of column
+// GATHER (grouped MUL_MAT_ID): column n of the image is the pair map.cols[n] of x (zeros for padding); the blocks of column
 // tiles past *map.ntt exit.  Each column's image is the one the dense instance writes for the same f32 column.
 template <bool GATHER>
 __global__ void __launch_bounds__(256) quantize_mmq32_kernel(const float * __restrict__ x, int64_t x_col_stride, int64_t ncols, int64_t k_valid,
@@ -73,21 +62,9 @@ __global__ void __launch_bounds__(256) quantize_mmq32_kernel(const float * __res
     const int64_t blk = blockIdx.x;
     const int64_t n = (int64_t)blockIdx.y * 8 + warp;                // token (padded range: < nt * 128)
     const int64_t nt = n >> 7; const int nl = (int)(n & 127);
+    if constexpr (GATHER) { if (nt >= *map.ntt) return; }            // the whole block: blockIdx.y / 16 is its column tile
     float v[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    if constexpr (GATHER) {
-        if (nt >= *map.ntt) return;                                  // the whole block: blockIdx.y / 16 is its column tile
-        const int pr = map.cols[n], nu = map.n_used;
-        if (pr >= 0) {
-            const int t = pr / nu, s = pr % nu;
-            const float4 * p = (const float4 *)(x + (int64_t)t * map.b_tok_stride + (s % map.n_b1) * map.b_slot_stride + blk * 256 + lane * 8);
-            const float4 a = p[0], b = p[1];
-            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-        }
-    } else if (n < ncols && blk * 256 + lane * 8 < k_valid) {
-        const float4 * p = (const float4 *)(x + n * x_col_stride + blk * 256 + lane * 8);
-        const float4 a = p[0], b = p[1];
-        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-    }
+    mmq_load_col8<GATHER>(v, x, x_col_stride, ncols, k_valid, map, n, blk * 256 + lane * 8);
     float am = 0.0f;
 #pragma unroll
     for (int j = 0; j < 8; j++) am = fmaxf(am, fabsf(v[j]));
@@ -103,21 +80,12 @@ __global__ void __launch_bounds__(256) quantize_mmq32_kernel(const float * __res
     pk.y = (q[4] & 0xff) | ((q[5] & 0xff) << 8) | ((q[6] & 0xff) << 16) | ((q[7] & 0xff) << 24);
     uint8_t * stage = ws + ((nt * g.ns + blk * 2 + (lane >> 4)) * T32_STAGE_B);
     const int b = (lane >> 2) & 3;                                   // block of the stage
-    *(uint2 *)(stage + (2 * b + ((lane & 3) >> 1)) * T32_PANEL + nl * 16 + (lane & 1) * 8) = pk;
-    if ((lane & 3) == 0) *(float *)(stage + 8 * T32_PANEL + (b * 128 + nl) * 4) = __half2float(__float2half_rn(d));   // the oracle stores d as f16
+    *(uint2 *)(stage + (2 * b + ((lane & 3) >> 1)) * MMQ_PANEL + nl * 16 + (lane & 1) * 8) = pk;
+    if ((lane & 3) == 0) *(float *)(stage + 8 * MMQ_PANEL + (b * 128 + nl) * 4) = __half2float(__float2half_rn(d));   // the oracle stores d as f16
     pdl_trigger();
 }
 
-struct Tc32Args {
-    const uint8_t * W;          // weights: repacked rows (repack_layout.cuh), k a multiple of 256 (padded rows included)
-    const uint8_t * ws;         // activation image (quantize_mmq32_kernel)
-    float *         dst;        // [ncols][ldd] f32
-    int64_t m, k, ncols, ldd, rb, nt;
-    int32_t ns, n_tiles;
-    unsigned long long * prof;  // per-role cycle counters of CTA 0 (B200_MMQ_PROF), normally null
-    MmidMap map;                // GROUPED only: W is the first expert's matrix, columns are (token, slot) pairs
-    int32_t n_mtiles;           // GROUPED only
-};
+using Tc32Args = MmqTileArgs;       // W: repacked rows (repack_layout.cuh), k a multiple of 256 (padded rows included); nks: 128-k stages
 
 struct Tc32Smem {
     static constexpr int A = 0, B = A + T32_NSTAGE * T32_STAGE_A;
@@ -130,10 +98,10 @@ __device__ __forceinline__ uint32_t bit4_of(uint32_t b) { return (((b & 0xFu) * 
 // bytes v in [0, 2 OFF) -> v - OFF as int8, four at a time (no borrow crosses a byte: 0x80 + v - OFF >= 0x70)
 template <uint32_t OFF> __device__ __forceinline__ uint32_t recentre(uint32_t v) { return ((v | 0x80808080u) - OFF * 0x01010101u) ^ 0x80808080u; }
 
-// GROUPED (MUL_MAT_ID, mmid.cuh): column tile ct multiplies expert map.tile_expert[ct]; the tile count comes from the device (*map.ntt)
+// GROUPED (MUL_MAT_ID): column tile ct multiplies expert map.tile_expert[ct]; the tile count comes from the device (*map.ntt)
 // and the epilogue scatters column j to its pair's output row (padding columns are not stored).  Everything else is the dense kernel.
 template <int T, bool GROUPED>
-__global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_constant__ Tc32Args args) {
+__global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc32_kernel(const __grid_constant__ Tc32Args args) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t * b_full = (uint64_t *)(smem + Tc32Smem::BAR), * a_full = b_full + T32_NSTAGE, * ab_empty = a_full + T32_NSTAGE;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -145,8 +113,8 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
     __syncthreads();
     pdl_wait();
 
-    const int ns = args.ns;
-    const auto NT = [&]() { if constexpr (GROUPED) return *args.map.ntt; else return args.nt; }();        // column tiles (grouped: 32-bit tile arithmetic)
+    const int ns = args.nks;
+    const auto NT = mmq_col_tiles<GROUPED>(args);
     const int n_tiles = GROUPED ? args.n_mtiles * (int)NT : args.n_tiles;
     unsigned long long w0 = 0, w1 = 0;                               // profile: cycles in this role's kinds of waits
     const bool prof = args.prof != nullptr && blockIdx.x == 0;
@@ -163,9 +131,7 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
         uint32_t it = 0;
         uint4 nxt[NQ], nxt_h = make_uint4(0, 0, 0, 0); uint2 nxt_d;
         auto fetch = [&](int tile, int s) {
-            int64_t r = (int64_t)(tile / NT) * T32_TM + t; if (r >= args.m) r = args.m - 1;   // rows past the end: any valid row (never stored)
-            const uint8_t * row = args.W + r * args.rb;
-            if constexpr (GROUPED) row += (int64_t)args.map.tile_expert[tile % NT] * args.map.expert_stride;
+            const uint8_t * row = mmq_weight_row<GROUPED>(args, tile / NT, tile % NT, t);
             const uint4 * p = (const uint4 *)(row + (int64_t)s * 4 * QB);
 #pragma unroll
             for (int i = 0; i < NQ; i++) nxt[i] = __ldg(p + i);
@@ -193,7 +159,7 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
                 uint8_t * As = smem + Tc32Smem::A + st * T32_STAGE_A + t * 16;
                 if (T == B200_TYPE_Q8_0) {
 #pragma unroll
-                    for (int c = 0; c < 8; c++) *(uint4 *)(As + c * T32_PANEL) = cur[c];
+                    for (int c = 0; c < 8; c++) *(uint4 *)(As + c * MMQ_PANEL) = cur[c];
                 } else {
                     const uint32_t qh[4] = { cur_h.x, cur_h.y, cur_h.z, cur_h.w };
 #pragma unroll
@@ -207,8 +173,8 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
                             if (T == B200_TYPE_Q4_0) { plo[i] = recentre<8>(l); phi[i] = recentre<8>(h); }
                             else { plo[i] = recentre<16>(l | bit4_of(qh[b] >> (4 * i))); phi[i] = recentre<16>(h | bit4_of(qh[b] >> (16 + 4 * i))); }   // qh bit j -> element j
                         }
-                        *(uint4 *)(As + (2 * b) * T32_PANEL) = lo;              // elements 0..15: low nibbles
-                        *(uint4 *)(As + (2 * b + 1) * T32_PANEL) = hi;          // elements 16..31: high nibbles
+                        *(uint4 *)(As + (2 * b) * MMQ_PANEL) = lo;              // elements 0..15: low nibbles
+                        *(uint4 *)(As + (2 * b + 1) * MMQ_PANEL) = hi;          // elements 16..31: high nibbles
                     }
                 }
                 float * rs = (float *)(smem + Tc32Smem::RS + st * 2048) + t;
@@ -235,16 +201,16 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
 #pragma unroll
             for (int c = 0; c < 32; c++) { f0[c] = 0; f1[c] = 0; }
             auto mma = [&](int32_t (&f)[32], int st, int b, int h) {
-                const uint32_t a = smem_u32(smem + Tc32Smem::A + st * T32_STAGE_A) + g * 1024 + b * 2 * T32_PANEL;
-                const uint32_t bb = smem_u32(smem + Tc32Smem::B + st * T32_STAGE_B) + h * 1024 + b * 2 * T32_PANEL;
+                const uint32_t a = smem_u32(smem + Tc32Smem::A + st * T32_STAGE_A) + g * 1024 + b * 2 * MMQ_PANEL;
+                const uint32_t bb = smem_u32(smem + Tc32Smem::B + st * T32_STAGE_B) + h * 1024 + b * 2 * MMQ_PANEL;
                 wg_fence();
-                wg_mma_ss_s8(f, wg_desc(a, T32_PANEL, 128u), wg_desc(bb, T32_PANEL, 128u), 0u);
+                wg_mma_ss_s8(f, wg_desc(a, MMQ_PANEL, 128u), wg_desc(bb, MMQ_PANEL, 128u), 0u);
                 wg_commit();
             };
             auto fold = [&](int32_t (&f)[32], int st, int b, int h) {
                 const float * rs = (const float *)(smem + Tc32Smem::RS + st * 2048) + b * 128;
                 const float da = rs[ra], db = rs[ra + 8];
-                const float2 * dx2 = (const float2 *)(smem + Tc32Smem::B + st * T32_STAGE_B + 8 * T32_PANEL + (b * 128 + 64 * h + c0) * 4);
+                const float2 * dx2 = (const float2 *)(smem + Tc32Smem::B + st * T32_STAGE_B + 8 * MMQ_PANEL + (b * 128 + 64 * h + c0) * 4);
 #pragma unroll
                 for (int j = 0; j < 8; j++) {
                     const float2 dxp = dx2[4 * j];
@@ -281,99 +247,35 @@ __global__ void __launch_bounds__(T32_THREADS, 1) mmq_tc32_kernel(const __grid_c
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&ab_empty[st]);                // every MMA and every scale read of the stage is done
             }
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int64_t row = mt * T32_TM + ra + 8 * h;
-                if (row >= args.m) continue;
-#pragma unroll
-                for (int j = 0; j < 16; j++) {
-#pragma unroll
-                    for (int e = 0; e < 2; e++) {
-                        const int64_t n = nt * T32_TN + 8 * j + c0 + e;
-                        if constexpr (GROUPED) {
-                            const int pr = args.map.cols[n], nu = args.map.n_used;
-                            if (pr >= 0) args.dst[(pr / nu) * args.map.dst_tok_stride + (pr % nu) * args.map.dst_slot_stride + row] = acc[4 * j + 2 * h + e];
-                        } else if (n < args.ncols) args.dst[n * args.ldd + row] = acc[4 * j + 2 * h + e];
-                    }
-                }
-            }
+            mmq_store_tile<GROUPED>(args, acc, mt, nt, ra, c0);
         }
     }
 
-    if (prof && lane == 0) {                                           // [warp][total, wait0, wait1, wait2]
-        unsigned long long * o = args.prof + warp * 4;
-        o[0] = (unsigned long long)(clock64() - t_start); o[1] = w0; o[2] = w1; o[3] = 0;
-    }
+    if (prof && lane == 0) mmq_prof_store(args, warp, t_start, w0, w1);
     pdl_trigger();
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
-// Fewest activation columns that go to the tensor cores; below it the columns stream through the matvec in groups of 8.  A tile pass
-// costs the same for 9 columns as for 128 (and a matrix of m rows occupies only m / 128 SMs), a column group costs one pass over the
-// weights.  Measured on the Llama-3-8B shapes at Q8_0 (H100.md): at 32 columns the column groups win on three shapes of four, at 64
-// the tensor cores win on all four; by the per-group time in between, 7 groups (49 columns) is where the tile kernel is ahead on all.
-#define T32_MIN_COLS 49
-
-bool b200_mmq_tc32_supported(int type, int64_t m, int64_t k, int64_t ncols) {
-    static const bool off = getenv("B200_MMQ_DISABLE_TC") != nullptr;     // comparison arm: column groups through the matvec kernel
-    return !off && type_is_block32(type) && m > 0 && ncols >= T32_MIN_COLS && k > 0 && k % 256 == 0;
-}
 int64_t b200_mmq_tc32_workspace(int64_t k, int64_t ncols) { return tc32_geom(k, ncols).total; }
 
-// grouped: a.n_tiles is the host's upper bound (the kernel reads the real count)
-template <int T, bool GROUPED = false> static int tc32_launch(const Tc32Args & a, cudaStream_t st) {
-    static bool attr[64] = { false };
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr[dev & 63]) { B200_CUDA(cudaFuncSetAttribute(mmq_tc32_kernel<T, GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, Tc32Smem::TOTAL)); attr[dev & 63] = true; }
-    const int grid = a.n_tiles < b200_sm_count() ? a.n_tiles : b200_sm_count();
-    B200_CUDA(b200_launch_pdl(mmq_tc32_kernel<T, GROUPED>, dim3((unsigned)grid), dim3(T32_THREADS), (size_t)Tc32Smem::TOTAL, st, a));
-    b200_count_launch();
-    return B200_OK;
+template <bool GROUPED> static int tc32_launch(int type, const Tc32Args & a, cudaStream_t st) {
+    switch (type) {
+        case B200_TYPE_Q4_0: return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_Q4_0, GROUPED>, Tc32Smem::TOTAL>(a, st);
+        case B200_TYPE_Q5_0: return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_Q5_0, GROUPED>, Tc32Smem::TOTAL>(a, st);
+        case B200_TYPE_Q8_0: return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_Q8_0, GROUPED>, Tc32Smem::TOTAL>(a, st);
+    }
+    return B200_ERR_UNSUPPORTED;
 }
 
-// k: length of the (padded) weight rows; k_valid <= k: elements that exist in X
-int b200_mmq_tc32(int type, const void * W, const float * X, int64_t x_col_stride, float * dst, int64_t ldd, int64_t m, int64_t k, int64_t k_valid, int64_t ncols, void * workspace, void * stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (((uintptr_t)W | (uintptr_t)X | (uintptr_t)workspace) & 15 || (x_col_stride & 3)) { b200_set_error("mul_mat_q: pointers must be 16-byte aligned"); return B200_ERR_INVALID; }
-    if (k_valid <= 0 || k_valid > k || k_valid % 8 != 0) { b200_set_error("mul_mat_q: k_valid must be a positive multiple of 8, at most k"); return B200_ERR_INVALID; }
-    const Tc32Geom g = tc32_geom(k, ncols);
+int b200_mmq_tc32(int type, const MmqJob & j, cudaStream_t st) {
+    const Tc32Geom g = tc32_geom(j.k, j.ncols);
     Tc32Args a = {};
-    a.W = (const uint8_t *)W; a.ws = (const uint8_t *)workspace; a.dst = dst; a.m = m; a.k = k; a.ncols = ncols; a.ldd = ldd;
-    a.rb = (k / 32) * type_block_bytes(type); a.nt = g.nt; a.ns = (int32_t)g.ns;
-    a.n_tiles = (int32_t)(((m + T32_TM - 1) / T32_TM) * g.nt);
-    a.prof = b200_mmq_prof_buf();
-    dim3 qgrid((unsigned)(k / 256), (unsigned)(g.nt * 16));
-    B200_CUDA(b200_launch_pdl(quantize_mmq32_kernel<false>, qgrid, dim3(256), 0, st, X, x_col_stride, ncols, k_valid, (uint8_t *)workspace, g, MmidMap{}));
+    mmq_tile_fill(a, j, (j.k / 32) * type_block_bytes(type));
+    a.nks = (int32_t)g.ns;
+    B200_CUDA(b200_launch_pdl(j.map ? quantize_mmq32_kernel<true> : quantize_mmq32_kernel<false>, dim3((unsigned)(j.k / 256), (unsigned)(a.nt * 16)), dim3(256), 0, st,
+                              j.X, j.x_col_stride, j.ncols, j.k_valid, (uint8_t *)j.workspace, g, a.map));
     b200_count_launch();
-    int rc = B200_ERR_UNSUPPORTED;
-    switch (type) {
-        case B200_TYPE_Q4_0: rc = tc32_launch<B200_TYPE_Q4_0>(a, st); break;
-        case B200_TYPE_Q5_0: rc = tc32_launch<B200_TYPE_Q5_0>(a, st); break;
-        case B200_TYPE_Q8_0: rc = tc32_launch<B200_TYPE_Q8_0>(a, st); break;
-    }
-    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc32", type, m, k, ncols, a.n_tiles, st);
-    return rc;
-}
-
-// grouped MUL_MAT_ID (mmid_route.cu): B f32 activations gathered through map, W the first expert, n_ct the upper bound of column tiles;
-// `image` (16-byte aligned) holds b200_mmq_tc32_workspace(k, 128 * n_ct) bytes
-int b200_mmq_tc32_grouped(int type, const void * W, const float * B, float * dst, int64_t m, int64_t k, int64_t n_ct, const MmidMap & map, void * image, cudaStream_t st) {
-    const Tc32Geom g = tc32_geom(k, n_ct * T32_TN);
-    Tc32Args a = {};
-    a.W = (const uint8_t *)W; a.ws = (const uint8_t *)image; a.dst = dst; a.m = m; a.k = k; a.ncols = n_ct * T32_TN;
-    a.rb = (k / 32) * type_block_bytes(type); a.nt = g.nt; a.ns = (int32_t)g.ns;
-    a.n_mtiles = (int32_t)((m + T32_TM - 1) / T32_TM); a.n_tiles = (int32_t)(a.n_mtiles * n_ct);
-    a.prof = b200_mmq_prof_buf();
-    a.map = map;
-    dim3 qgrid((unsigned)(k / 256), (unsigned)(n_ct * 16));
-    B200_CUDA(b200_launch_pdl(quantize_mmq32_kernel<true>, qgrid, dim3(256), 0, st, B, (int64_t)0, a.ncols, k, (uint8_t *)image, g, map));
-    b200_count_launch();
-    int rc = B200_ERR_UNSUPPORTED;
-    switch (type) {
-        case B200_TYPE_Q4_0: rc = tc32_launch<B200_TYPE_Q4_0, true>(a, st); break;
-        case B200_TYPE_Q5_0: rc = tc32_launch<B200_TYPE_Q5_0, true>(a, st); break;
-        case B200_TYPE_Q8_0: rc = tc32_launch<B200_TYPE_Q8_0, true>(a, st); break;
-    }
-    if (a.prof && rc == B200_OK) b200_mmq_prof_report("mmq_tc32 grouped", type, m, k, a.ncols, a.n_tiles, st);
+    const int rc = j.map ? tc32_launch<true>(type, a, st) : tc32_launch<false>(type, a, st);
+    if (a.prof && rc == B200_OK) mmq_prof_report(j.map ? "mmq_tc32 grouped" : "mmq_tc32", type, a, st);
     return rc;
 }

@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 
 TYPES = [Q4_0, Q5_0, Q8_0]
-MIN_COLS = 49           # T32_MIN_COLS of mmq_tc32.cu: fewer columns stream through the matvec in groups of 8
+MIN_COLS = 49           # T32_MIN_COLS of mmq.cu: fewer columns stream through the matvec in groups of 8
 
 
 def dev(a):
