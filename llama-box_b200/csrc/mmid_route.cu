@@ -45,6 +45,8 @@ RouteGeom route_geom(int type, int64_t k, int64_t n_expert, int64_t n_used, int6
 }
 
 bool mmid_tc_ok(int type, int64_t m, int64_t k, int64_t n_expert, int64_t n_used, int64_t n_tok) {
+    // the tuned six only: the K-quant kernel also takes Q2_K / Q3_K, but as dense MUL_MAT (no grouped instance)
+    if (!(type_is_block32(type) || type == B200_TYPE_Q4_K || type == B200_TYPE_Q5_K || type == B200_TYPE_Q6_K)) return false;
     if (!mmq_tile_takes(type, m, k)) return false;
     if (n_tok < MMID_MIN_TOK || n_expert <= 0 || n_expert > MMID_MAX_EXPERT || n_used <= 0 || n_used > n_expert) return false;
     if (n_tok * n_used > INT32_MAX / 2 || n_tok * n_used < MMID_MIN_PAIRS * n_expert) return false;

@@ -14,7 +14,9 @@
 //     6-bit sub-block scale folded in, a[r][k] = sc_j * q  (<= 63*15 = 945 for Q4_K, <= 63*31 = 1953 for Q5_K: exact in f16),
 //     written as K-major core matrices.  Q6_K's sc * (q - 32) reaches +-4096, which f16 holds only when even: the
 //     product is split as (sc & ~1) * (q - 32)  [even, exact]  +  (sc & 1) * (q - 32)  [|.| <= 32], two K-passes into ONE
-//     accumulator.
+//     accumulator.  Q2_K (sc * q <= 15 * 3, a 4-bit min per 16 elements) and Q3_K ((sc - 32) * q with q in [-4, 3]: |.| <= 128, no
+//     min) are read in ggml's native block layout, which decode (ext_mmv_kernel) and GET_ROWS share: 84 B / 110 B per block, so only
+//     4-byte / 2-byte aligned, loaded as 32-bit words (Q3_K: from the aligned word below the block, realigned with funnel shifts).
 //   * B operand (activations): q8 values as f16 integers (|q8| <= 127), pre-tiled in HBM in the exact shared-memory image so
 //     that one bulk copy brings a [128 tokens x 64 k] panel.
 //   * wgmma m64n128k16 f16, f32 accumulate in registers: every product and every partial sum is an integer below 2^24, so the
@@ -32,6 +34,7 @@
 // Shared memory (per CTA, ~150 KB): 2 A stages x 32 KB (128 rows x 128 k f16) + 2 B stages x 32 KB + the imin operands + scale rings.
 // Data movement: weights are read from HBM once per 128-token tile (L2 serves the other token tiles of the same rows, which
 // run on neighbouring CTAs), activations stream from L2.
+#include "extfmt.cuh"
 #include "mmq_tile.cuh"
 #include "wgmma.cuh"
 
@@ -120,6 +123,8 @@ template <int T> struct TcType;
 template <> struct TcType<B200_TYPE_Q4_K> { static constexpr int STAGES = 2, HAS_MIN = 1, B_BYTES = 32768; };
 template <> struct TcType<B200_TYPE_Q5_K> { static constexpr int STAGES = 2, HAS_MIN = 1, B_BYTES = 32768; };
 template <> struct TcType<B200_TYPE_Q6_K> { static constexpr int STAGES = 4, HAS_MIN = 0, B_BYTES = 16384; };
+template <> struct TcType<B200_TYPE_Q2_K> { static constexpr int STAGES = 2, HAS_MIN = 1, B_BYTES = 32768; };
+template <> struct TcType<B200_TYPE_Q3_K> { static constexpr int STAGES = 2, HAS_MIN = 0, B_BYTES = 32768; };
 
 // shared memory map
 struct TcSmem {
@@ -136,6 +141,8 @@ __device__ __forceinline__ uint32_t hfma2_u(uint32_t a, uint32_t b, uint32_t c) 
 __device__ __forceinline__ uint32_t hmul2_u(uint32_t a, uint32_t b) { uint32_t d; asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t hsub2_u(uint32_t a, uint32_t b) { uint32_t d; asm("sub.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t h2_of_int(int v) { const uint32_t h = __half_as_ushort(__int2half_rn(v)); return h | (h << 16); }
+// bytes 0, 1 (hi: 2, 3) of v, each < 1024, as an f16 pair (exact)
+__device__ __forceinline__ uint32_t h2_of_bytes(uint32_t v, bool hi) { return hsub2_u(__byte_perm(v, 0u, hi ? 0x4342u : 0x4140u) | 0x64006400u, 0x64006400u); }
 
 // 6-bit scales / mins of a q4_K / q5_K block header (ggml-quants.c:703-711), all 8 at once
 __device__ __forceinline__ void k4_unpack(uint32_t y, uint32_t z, uint32_t w, uint32_t & sc03, uint32_t & sc47, uint32_t & mn03, uint32_t & mn47) {
@@ -191,15 +198,30 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc_kernel(const __grid_con
         // the current one).  (A first version staged the blocks through shared memory with one cp.async.bulk per row: a
         // warp-wide bulk copy is issued lane by lane through uniform registers, ~65 cycles each — 128 rows cost 8 K cycles per
         // super-block and starved everything else.)
-        constexpr int NW = T == B200_TYPE_Q4_K ? 9 : (T == B200_TYPE_Q5_K ? 11 : 13);
+        // (Q2_K: 21 32-bit words; Q3_K: 28, from the aligned word at or below the block start, whose offset in it is nxt_sh bytes)
+        constexpr int NW = T == B200_TYPE_Q4_K ? 9 : T == B200_TYPE_Q5_K ? 11 : T == B200_TYPE_Q6_K ? 13 : T == B200_TYPE_Q2_K ? 6 : 7;
         const int t = tid - 8 * 32;                                      // weight row of the tile
         const int64_t nb = args.k / 256;
         uint32_t it = 0, sbc = 0;
-        uint4 nxt[NW]; uint16_t nxt_d = 0;
+        uint4 nxt[NW]; uint16_t nxt_d = 0; uint32_t nxt_sh = 0;
         auto fetch = [&](int tile, int sb) {
             const int64_t mt = tile / NT;
             const uint8_t * row = mmq_weight_row<GROUPED>(args, mt, tile - mt * NT, t);
-            if (T == B200_TYPE_Q6_K) {
+            auto ld16b = [](const uint8_t * p) { return make_uint4(ldg_nc32(p), ldg_nc32(p + 4), ldg_nc32(p + 8), ldg_nc32(p + 12)); };
+            if constexpr (T == B200_TYPE_Q2_K) {
+                const uint8_t * p = row + (int64_t)sb * 84;                  // 4-byte aligned
+#pragma unroll
+                for (int i = 0; i < 5; i++) nxt[i] = ld16b(p + 16 * i);
+                nxt[5] = make_uint4(ldg_nc32(p + 80), 0u, 0u, 0u);
+            } else if constexpr (T == B200_TYPE_Q3_K) {
+                const uint8_t * b = row + (int64_t)sb * 110;                 // 2-byte aligned
+                nxt_sh = (uint32_t)(uintptr_t)b & 2u;
+                const uint8_t * p = b - nxt_sh;
+#pragma unroll
+                for (int i = 0; i < 6; i++) nxt[i] = ld16b(p + 16 * i);
+                // the last word: 16 bits where the block ends inside it (never reads past the block, so never past the matrix)
+                nxt[6] = make_uint4(ldg_nc32(p + 96), ldg_nc32(p + 100), ldg_nc32(p + 104), nxt_sh ? ldg_nc32(p + 108) : (uint32_t)ldg_nc16(p + 108));
+            } else if (T == B200_TYPE_Q6_K) {
                 const uint4 * ql = (const uint4 *)(row + (int64_t)sb * 128), * qh = (const uint4 *)(row + nb * 128 + (int64_t)sb * 64);
 #pragma unroll
                 for (int i = 0; i < 8; i++) nxt[i] = __ldg(ql + i);
@@ -217,7 +239,7 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc_kernel(const __grid_con
         for (int tile = blockIdx.x; tile < n_tiles(); tile += gridDim.x) {
             for (int sb = 0; sb < nsb; sb++, sbc++) {
                 const int rs = sbc & 1;                                  // accumulator / imin-operand slot
-                uint4 cur[NW]; const uint16_t cur_d = nxt_d;
+                uint4 cur[NW]; const uint16_t cur_d = nxt_d; const uint32_t cur_sh = nxt_sh;
 #pragma unroll
                 for (int i = 0; i < NW; i++) cur[i] = nxt[i];
                 {   // prefetch the next super-block (of this tile, or the first one of this CTA's next tile)
@@ -226,7 +248,70 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc_kernel(const __grid_con
                     if (ntile < n_tiles()) fetch(ntile, nsbi);
                 }
                 float2 * rscale = (float2 *)(smem + TcSmem::RS + (sbc & 3) * 1024);
-                if (T == B200_TYPE_Q4_K || T == B200_TYPE_Q5_K) {
+                if constexpr (T == B200_TYPE_Q2_K || T == B200_TYPE_Q3_K) {
+                    // ---- Q2_K {scales[16], qs[64], d, dmin} / Q3_K {hmask[32], qs[64], scales[12], d} (ggml-quants.c dequantize_row_q2_K / _q3_K):
+                    // element 128 n + 32 j + l is the 2-bit field 2 j of qs[32 n + l] (Q3_K: plus 4 x bit 4 n + j of hmask[l], minus 4); its
+                    // scale (Q2_K: and min) is that of its 16-element group.  Half n is stage s = n.
+                    auto raw = [&](int i) { const uint4 & v = cur[i >> 2]; return (i & 3) == 0 ? v.x : (i & 3) == 1 ? v.y : (i & 3) == 2 ? v.z : v.w; };
+                    auto word = [&](int i) { return T == B200_TYPE_Q2_K ? raw(i) : __funnelshift_r(raw(i), raw(i + 1), 8 * cur_sh); };   // 32-bit word i of the block
+                    constexpr int QS = T == B200_TYPE_Q2_K ? 4 : 8;               // first word of qs
+                    const uint32_t sc12[3] = { word(24), word(25), word(26) };      // Q3_K: the 12 packed scale bytes (registers once inlined)
+#pragma unroll
+                    for (int s = 0; s < 2; s++, it++) {
+                        const int st = it & 1;
+                        mbar_wait_p(&ab_empty[st], ((it >> 1) & 1) ^ 1, pw1);
+                        if (t == 0) load_b(tile % NT, sb, sbc, s, st);
+                        uint8_t * As = smem + TcSmem::A + st * TC_STAGE_A + t * 16;
+#pragma unroll
+                        for (int j = 0; j < 4; j++) {                     // 32-element group j: K-chunks 4 j .. 4 j + 3 of the stage
+#pragma unroll
+                            for (int i = 0; i < 4; i++) {                 // l = 8 i .. 8 i + 7: qs words QS + 8 s + 2 i + u, hmask words 2 i + u
+                                const int g = 8 * s + 2 * j + (i >> 1);
+                                uint4 o;
+                                uint32_t * po = (uint32_t *)&o;
+                                if constexpr (T == B200_TYPE_Q2_K) {
+                                    const int sc = (int)(word(g >> 2) >> (8 * (g & 3))) & 15;
+                                    const uint32_t m = h2_of_int(sc), c = h2_of_int(-1024 * sc);
+#pragma unroll
+                                    for (int u = 0; u < 2; u++) {
+                                        const uint32_t qw = word(QS + 8 * s + 2 * i + u);
+                                        const uint32_t x0 = ((qw >> (2 * j)) & 0x00030003u) | 0x64006400u;                  // 1024 + q, elements (e, e+2)
+                                        const uint32_t x1 = ((qw >> (2 * j + 8)) & 0x00030003u) | 0x64006400u;              // elements (e+1, e+3)
+                                        po[2 * u] = hfma2_u(x0, m, c); po[2 * u + 1] = hfma2_u(x1, m, c);                  // exact: sc * q
+                                    }
+                                } else {
+                                    const uint32_t m = h2_of_int(xf_q3k_scale((const uint8_t *)sc12, g));
+#pragma unroll
+                                    for (int u = 0; u < 2; u++) {
+                                        const uint32_t qw = word(QS + 8 * s + 2 * i + u), hw = word(2 * i + u);
+                                        const uint32_t x0 = ((qw >> (2 * j)) & 0x00030003u) | (((hw >> (4 * s + j)) & 0x00010001u) << 2) | 0x64006400u;
+                                        const uint32_t x1 = ((qw >> (2 * j + 8)) & 0x00030003u) | (((hw >> (4 * s + j + 8)) & 0x00010001u) << 2) | 0x64006400u;
+                                        // (1024 + q2 + 4 h) - 1028 = q in [-4, 3], then (sc - 32) * q: both exact (|.| <= 128)
+                                        po[2 * u] = hmul2_u(hsub2_u(x0, 0x64046404u), m); po[2 * u + 1] = hmul2_u(hsub2_u(x1, 0x64046404u), m);
+                                    }
+                                }
+                                *(uint4 *)(As + (4 * j + i) * MMQ_PANEL) = o;
+                            }
+                        }
+                        if (s == 0) {
+                            if constexpr (T == B200_TYPE_Q2_K) {
+                                // imin operand: m_0 .. m_15 in natural order, the order of the quantiser's bsum panel; d, dmin for the epilogue
+                                uint8_t * Am = smem + TcSmem::AM + rs * 4096 + t * 16;
+                                uint32_t mn[4];
+#pragma unroll
+                                for (int w = 0; w < 4; w++) mn[w] = (word(w) >> 4) & 0x0F0F0F0Fu;
+                                *(uint4 *)Am = make_uint4(h2_of_bytes(mn[0], false), h2_of_bytes(mn[0], true), h2_of_bytes(mn[1], false), h2_of_bytes(mn[1], true));
+                                *(uint4 *)(Am + MMQ_PANEL) = make_uint4(h2_of_bytes(mn[2], false), h2_of_bytes(mn[2], true), h2_of_bytes(mn[3], false), h2_of_bytes(mn[3], true));
+                                rscale[t] = make_float2(h2f((uint16_t)(word(20) & 0xffff)), h2f((uint16_t)(word(20) >> 16)));
+                            } else {
+                                rscale[t] = make_float2(h2f((uint16_t)(raw(27) >> (8 * cur_sh))), 0.0f);
+                            }
+                        }
+                        fence_async_smem();
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&a_full[st]);
+                    }
+                } else if (T == B200_TYPE_Q4_K || T == B200_TYPE_Q5_K) {
                     constexpr int QW = T == B200_TYPE_Q4_K ? 1 : 3;       // first 16-byte word of qs
                     const uint4 hdr = cur[0];
                     uint32_t sc03, sc47, mn03, mn47;
@@ -406,13 +491,16 @@ template <bool GROUPED> static int tc_launch(int type, const TcArgs & a, cudaStr
         case B200_TYPE_Q4_K: return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q4_K, GROUPED>, TcSmem::TOTAL>(a, st);
         case B200_TYPE_Q5_K: return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q5_K, GROUPED>, TcSmem::TOTAL>(a, st);
         case B200_TYPE_Q6_K: return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q6_K, GROUPED>, TcSmem::TOTAL>(a, st);
+        // dense only: MUL_MAT_ID on these formats stays on the matvec (mmid_route.cu)
+        case B200_TYPE_Q2_K: if constexpr (!GROUPED) return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q2_K, false>, TcSmem::TOTAL>(a, st); break;
+        case B200_TYPE_Q3_K: if constexpr (!GROUPED) return mmq_tile_launch<mmq_tc_kernel<B200_TYPE_Q3_K, false>, TcSmem::TOTAL>(a, st); break;
     }
     return B200_ERR_UNSUPPORTED;
 }
 
 int b200_mmq_tc(int type, const MmqJob & j, cudaStream_t st) {
     TcArgs a = {};
-    mmq_tile_fill(a, j, (j.k / 256) * type_block_bytes(type));
+    mmq_tile_fill(a, j, (j.k / 256) * xf_block_bytes(type));          // Q6_K's repacked rows are as long as its native ones
     a.g = tc_geom(j.k, j.ncols);
     a.nks = (int32_t)(j.k / 256);
     a.lbo = (uint32_t)MMQ_PANEL; a.sbo = 128u;
