@@ -675,8 +675,8 @@ struct Runner {
             // a format only the wide matvec reads (mmvq_ext.cu): f32 activations in, quantised inside the kernel; one pass over the weights per column
             { const int fs = mk_flush(); if (fs != B200_OK) return fs; }
             invalidate_act(n.dst);
-            if (b200_mul_mat_q_workspace(w.type, m, kv, ncols) > 0) {    // Q2_K / Q3_K prefill: the K-quant tensor-core GEMM (mmq_tc.cu)
-                ex->act_id[0] = ex->act_id[1] = 0;                       // its activation image goes to the q8_K act buffer
+            if (b200_mul_mat_q_workspace(w.type, m, kv, ncols) > 0) {    // Q2_K / Q3_K / IQ4_NL / IQ4_XS prefill: a tensor-core GEMM (mmq_tc.cu / mmq_tc32.cu)
+                ex->act_id[0] = ex->act_id[1] = 0;                       // its activation image goes to the q8_K act buffer (plan_workspace sized it)
                 return KL(b200_mul_mat_q2(w.type, w.data, (const float *)x.data, x.nb[1] / 4, (float *)n.dst.data, n.dst.nb[1] / 4, m, kv, kv, ncols, act_buf(0), st));
             }
             return KL(b200_mul_mat_vec_wide(w.type, w.data, (const float *)x.data, x.nb[1] / 4, (float *)n.dst.data, n.dst.nb[1] / 4, nullptr, nullptr, m, kv, ncols, st));
@@ -1028,7 +1028,7 @@ int plan_workspace(b200_executor * ex, const b200_node * nodes, int n) {
                 const size_t b = (size_t)b200_mul_mat_q_workspace(nd.src[0].type, nd.src[0].ne[1], k, cols);
                 if (kd >= 0 && b > act[kd]) act[kd] = b;
             }
-            if (wide_on() && is_wide_only_type(nd.src[0].type)) {   // Q2_K / Q3_K prefill on the tensor cores: the image in the q8_K act buffer
+            if (wide_on() && is_wide_only_type(nd.src[0].type)) {   // Q2_K / Q3_K / IQ4_NL / IQ4_XS prefill on the tensor cores: the image in the q8_K act buffer
                 const size_t b = (size_t)b200_mul_mat_q_workspace(nd.src[0].type, nd.src[0].ne[1], nd.src[0].ne[0], cols);
                 if (b > act[0]) act[0] = b;
             }

@@ -131,6 +131,10 @@ XF_HD int xf_q3k_scale(const uint8_t * sc12, int g) {                     // sc1
     return (int)(int8_t)(w >> (8 * (g & 3))) - 32;
 }
 
+// 6-bit scale ls of sub-block ib (0..7) of an IQ4_XS super-block (ggml-quants.c dequantize_row_iq4_xs): scl holds its scales_l byte
+// scales_l[ib / 2] in the low 8 bits (higher bits are ignored), sch the 16-bit scales_h (higher bits are ignored)
+XF_HD int xf_iq4xs_ls(int scl, uint32_t sch, int ib) { return (int)((scl >> (4 * (ib & 1))) & 0xF) | (int)(((sch >> (2 * ib)) & 3) << 4); }
+
 // ---- the quantised activation column a sub-block is multiplied with ------------------------------------------------------
 //   family 1 (32-wide, q8_0 / q8_1 of the x86 CPU backend, ggml-cpu/arch/x86/quants.c:290-492):
 //       qs[k] int8 | d[k/32] = value of the f16-rounded scale | s[k/32] = value of f16(d_unrounded * sum)  (q8_1 only) | bs[k/32] = sum of the 32 quants
@@ -311,7 +315,7 @@ template <> XF_HD float xf_sub_dot<XF_IQ4_XS>(const uint8_t * row, int64_t, int6
     const uint8_t * b = row + sb * 136;
     const uint32_t * a = (const uint32_t *)(A.qs + u * 32);
     const uint32_t hd = xf_ld32(b);                                           // d | scales_h << 16
-    const int ls = (int)((b[4 + (s >> 1)] >> (4 * (s & 1))) & 0xF) | (int)((((hd >> 16) >> (2 * s)) & 3) << 4);
+    const int ls = (int)((b[4 + (s >> 1)] >> (4 * (s & 1))) & 0xF) | (int)((((hd >> 16) >> (2 * s)) & 3) << 4);    // xf_iq4xs_ls written out (the call reorders this kernel's registers)
     int sumi = 0;
     for (int i = 0; i < 4; i++) {
         const uint32_t w = xf_ld32(b + 8 + 16 * s + 4 * i);
@@ -427,7 +431,7 @@ template <> XF_HD void xf_sub_dequant<XF_Q6_K>(const uint8_t * row, int64_t nb, 
 template <> XF_HD void xf_sub_dequant<XF_IQ4_XS>(const uint8_t * row, int64_t, int64_t u, float * y) {
     const int64_t sb = u >> 3; const int s = (int)(u & 7);
     const uint8_t * b = row + sb * 136; const float d = xf_h2f((uint16_t)xf_ld16(b)); const uint32_t sh = xf_ld16(b + 2);
-    const int ls = (int)((b[4 + (s >> 1)] >> (4 * (s & 1))) & 0xF) | (int)(((sh >> (2 * s)) & 3) << 4);
+    const int ls = xf_iq4xs_ls(b[4 + (s >> 1)], sh, s);
     const float dl = xf_mul(d, (float)(ls - 32));
     for (int jj = 0; jj < 16; jj++) { y[jj] = xf_mul(dl, (float)xf_kv_iq4nl(b[8 + 16 * s + jj] & 0xF)); y[jj + 16] = xf_mul(dl, (float)xf_kv_iq4nl(b[8 + 16 * s + jj] >> 4)); }
 }

@@ -29,7 +29,15 @@
 //     warps 8-11       transform: thread t owns weight row t of the tile, reads its packed blocks one stage ahead from global
 //                      memory into registers; thread 0 also issues the activation panel of each stage (cp.async.bulk)
 // A stage is 128 k (4 blocks): A 16 KB (int8 core matrices) + B 16 KB + d_x 2 KB + d_w 2 KB; 4 stages, ~144 KB of shared memory.
+//
+// IQ4_NL / IQ4_XS (the wide path's non-linear 4-bit formats, dense MUL_MAT only) are read in ggml's native block layout; the transform
+// looks each nibble up in kvalues_iq4nl (int8 in [-127, 113]) and places it like Q4_0 (mmq_wide32.cuh), so one IGMMA is still one
+// block's exact integer sum.  IQ4_NL has q8_0 activations and folds like Q8_0; IQ4_XS has q8_K activations (one f32 d_x per 256
+// elements, written to the image for each block, not f16-rounded) and a 6-bit scale per block, folded as the oracle does:
+//
+//     IQ4_XS:        acc += ((d_w * d_x) * (float)(ls - 32)) * (float)s
 #include "mmq_tile.cuh"
+#include "mmq_wide32.cuh"
 #include "wgmma.cuh"
 
 #define T32_KS 128                  // k per stage
@@ -85,6 +93,40 @@ __global__ void __launch_bounds__(256) quantize_mmq32_kernel(const float * __res
     pdl_trigger();
 }
 
+// IQ4_XS: the same image from q8_K activations (quantize_row_q8_K_ref, as quantize_mmq_kernel of mmq_tc.cu does it), one warp per
+// (token, super-block); d_x is the super-block's f32 d, written for each of the 4 blocks of both its stages.  Dense only.
+__global__ void __launch_bounds__(256) quantize_mmq32k_kernel(const float * __restrict__ x, int64_t x_col_stride, int64_t ncols, int64_t k_valid,
+                                                             uint8_t * __restrict__ ws, Tc32Geom g) {
+    pdl_wait();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t sb = blockIdx.x;
+    const int64_t n = (int64_t)blockIdx.y * 8 + warp;                // token (padded range: < nt * 128)
+    const int64_t nt = n >> 7; const int nl = (int)(n & 127);
+    float v[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
+    const MmidMap none = {};
+    mmq_load_col8<false>(v, x, x_col_stride, ncols, k_valid, none, n, sb * 256 + lane * 8);
+    float am = 0.0f; int ai = 0;
+#pragma unroll
+    for (int j = 0; j < 8; j++) { const float a = fabsf(v[j]); if (a > am) { am = a; ai = lane * 8 + j; } }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {                               // the first index of the largest |x|
+        const float am2 = __shfl_xor_sync(0xffffffffu, am, o);
+        const int   ai2 = __shfl_xor_sync(0xffffffffu, ai, o);
+        if (am2 > am || (am2 == am && ai2 < ai)) { am = am2; ai = ai2; }
+    }
+    float mine = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 8; j++) if ((ai & 7) == j) mine = v[j];
+    const float maxv = __shfl_sync(0xffffffffu, mine, ai >> 3);
+    uint2 pk;
+    const float d = w32_q8k_quant8(v, maxv, am, pk.x, pk.y);
+    uint8_t * stage = ws + ((nt * g.ns + sb * 2 + (lane >> 4)) * T32_STAGE_B);
+    const int b = (lane >> 2) & 3;                                   // block of the stage
+    *(uint2 *)(stage + (2 * b + ((lane & 3) >> 1)) * MMQ_PANEL + nl * 16 + (lane & 1) * 8) = pk;
+    if ((lane & 3) == 0) *(float *)(stage + 8 * MMQ_PANEL + (b * 128 + nl) * 4) = d;
+    pdl_trigger();
+}
+
 using Tc32Args = MmqTileArgs;       // W: repacked rows (repack_layout.cuh), k a multiple of 256 (padded rows included); nks: 128-k stages
 
 struct Tc32Smem {
@@ -124,19 +166,25 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc32_kernel(const __grid_c
     if (warp >= 8) {
         // ===================== transform: packed blocks -> int8 core matrices + d_w =====================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 88;");
+        constexpr bool IQ4 = T == B200_TYPE_IQ4_NL || T == B200_TYPE_IQ4_XS;  // native blocks, one stage as 9 aligned 8-byte words (mmq_wide32.cuh)
         constexpr int NQ = T == B200_TYPE_Q8_0 ? 8 : 4;                  // 16-byte words of qs per row and stage
         constexpr int QB = T == B200_TYPE_Q8_0 ? 32 : 16;                // qs bytes per block
         const int t = tid - 8 * 32;                                      // weight row of the tile
         const int64_t nb = args.k / 32;
         uint32_t it = 0;
         uint4 nxt[NQ], nxt_h = make_uint4(0, 0, 0, 0); uint2 nxt_d;
+        uint32_t nxt_w[18];
         auto fetch = [&](int tile, int s) {
             const uint8_t * row = mmq_weight_row<GROUPED>(args, tile / NT, tile % NT, t);
-            const uint4 * p = (const uint4 *)(row + (int64_t)s * 4 * QB);
+            if constexpr (IQ4) {
+                w32_load<T>(row, s, nxt_w);
+            } else {
+                const uint4 * p = (const uint4 *)(row + (int64_t)s * 4 * QB);
 #pragma unroll
-            for (int i = 0; i < NQ; i++) nxt[i] = __ldg(p + i);
-            if (T == B200_TYPE_Q5_0) nxt_h = __ldg((const uint4 *)(row + nb * 16 + (int64_t)s * 16));
-            nxt_d = __ldg((const uint2 *)(row + nb * (T == B200_TYPE_Q5_0 ? 20 : QB) + (int64_t)s * 8));
+                for (int i = 0; i < NQ; i++) nxt[i] = __ldg(p + i);
+                if (T == B200_TYPE_Q5_0) nxt_h = __ldg((const uint4 *)(row + nb * 16 + (int64_t)s * 16));
+                nxt_d = __ldg((const uint2 *)(row + nb * (T == B200_TYPE_Q5_0 ? 20 : QB) + (int64_t)s * 8));
+            }
         };
         if (blockIdx.x < n_tiles) fetch(blockIdx.x, 0);
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -144,6 +192,11 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc32_kernel(const __grid_c
                 uint4 cur[NQ]; const uint4 cur_h = nxt_h; const uint2 cur_d = nxt_d;
 #pragma unroll
                 for (int i = 0; i < NQ; i++) cur[i] = nxt[i];
+                uint32_t cur_w[18];
+                if constexpr (IQ4) {
+#pragma unroll
+                    for (int i = 0; i < 18; i++) cur_w[i] = nxt_w[i];
+                }
                 {   // prefetch the next stage (of this tile, or the first one of this CTA's next tile)
                     int ntile = tile, nsi = s + 1;
                     if (nsi == ns) { nsi = 0; ntile = tile + gridDim.x; }
@@ -157,7 +210,18 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc32_kernel(const __grid_c
                     for (int o = 0; o < T32_STAGE_B; o += T32_STAGE_B / 3) bulk_g2s(smem + Tc32Smem::B + st * T32_STAGE_B + o, src + o, T32_STAGE_B / 3, &b_full[st]);
                 }
                 uint8_t * As = smem + Tc32Smem::A + st * T32_STAGE_A + t * 16;
-                if (T == B200_TYPE_Q8_0) {
+                if constexpr (IQ4) {
+                    float * rs = (float *)(smem + Tc32Smem::RS + st * 2048) + t;
+#pragma unroll
+                    for (int b = 0; b < 4; b++) {
+                        uint32_t q[8];
+                        const uint32_t sc = w32_unpack<T>(cur_w, s, b, q);
+                        *(uint4 *)(As + (2 * b) * MMQ_PANEL) = make_uint4(q[0], q[1], q[2], q[3]);         // elements 0..15: low nibbles
+                        *(uint4 *)(As + (2 * b + 1) * MMQ_PANEL) = make_uint4(q[4], q[5], q[6], q[7]);     // elements 16..31: high nibbles
+                        if (T == B200_TYPE_IQ4_NL) rs[128 * b] = h2f((uint16_t)sc);
+                        else ((uint32_t *)rs)[128 * b] = sc;                                               // d_w bits | (ls - 32) << 16
+                    }
+                } else if (T == B200_TYPE_Q8_0) {
 #pragma unroll
                     for (int c = 0; c < 8; c++) *(uint4 *)(As + c * MMQ_PANEL) = cur[c];
                 } else {
@@ -177,9 +241,11 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc32_kernel(const __grid_c
                         *(uint4 *)(As + (2 * b + 1) * MMQ_PANEL) = hi;          // elements 16..31: high nibbles
                     }
                 }
-                float * rs = (float *)(smem + Tc32Smem::RS + st * 2048) + t;
-                rs[0]   = h2f((uint16_t)(cur_d.x & 0xffff)); rs[128] = h2f((uint16_t)(cur_d.x >> 16));
-                rs[256] = h2f((uint16_t)(cur_d.y & 0xffff)); rs[384] = h2f((uint16_t)(cur_d.y >> 16));
+                if constexpr (!IQ4) {
+                    float * rs = (float *)(smem + Tc32Smem::RS + st * 2048) + t;
+                    rs[0]   = h2f((uint16_t)(cur_d.x & 0xffff)); rs[128] = h2f((uint16_t)(cur_d.x >> 16));
+                    rs[256] = h2f((uint16_t)(cur_d.y & 0xffff)); rs[384] = h2f((uint16_t)(cur_d.y >> 16));
+                }
                 fence_async_smem();                                       // generic-proxy writes -> visible to the tensor core (async proxy)
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&a_full[st]);
@@ -222,7 +288,12 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) mmq_tc32_kernel(const __grid_c
                         if (T == B200_TYPE_Q4_0) {                                  // ((float)s * d_w) * d_x
                             ua = __fadd_rn(ua, __fmul_rn(__fmul_rn(sa, da), dx));
                             ub = __fadd_rn(ub, __fmul_rn(__fmul_rn(sb, db), dx));
-                        } else {                                                    // (float)s * (d_w * d_x)
+                        } else if (T == B200_TYPE_IQ4_XS) {                         // ((d_w * d_x) * (float)(ls - 32)) * (float)s
+                            const uint32_t wa = __float_as_uint(da), wb = __float_as_uint(db);
+                            const float la = (float)((int32_t)wa >> 16), lb = (float)((int32_t)wb >> 16);
+                            ua = __fadd_rn(ua, __fmul_rn(__fmul_rn(__fmul_rn(h2f((uint16_t)wa), dx), la), sa));
+                            ub = __fadd_rn(ub, __fmul_rn(__fmul_rn(__fmul_rn(h2f((uint16_t)wb), dx), lb), sb));
+                        } else {                                                    // Q5_0 / Q8_0 / IQ4_NL: (float)s * (d_w * d_x)
                             ua = __fadd_rn(ua, __fmul_rn(sa, __fmul_rn(da, dx)));
                             ub = __fadd_rn(ub, __fmul_rn(sb, __fmul_rn(db, dx)));
                         }
@@ -263,6 +334,9 @@ template <bool GROUPED> static int tc32_launch(int type, const Tc32Args & a, cud
         case B200_TYPE_Q4_0: return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_Q4_0, GROUPED>, Tc32Smem::TOTAL>(a, st);
         case B200_TYPE_Q5_0: return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_Q5_0, GROUPED>, Tc32Smem::TOTAL>(a, st);
         case B200_TYPE_Q8_0: return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_Q8_0, GROUPED>, Tc32Smem::TOTAL>(a, st);
+        // dense only: MUL_MAT_ID on these formats stays on the wide matvec (mmid_route.cu)
+        case B200_TYPE_IQ4_NL: if constexpr (!GROUPED) return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_IQ4_NL, false>, Tc32Smem::TOTAL>(a, st); break;
+        case B200_TYPE_IQ4_XS: if constexpr (!GROUPED) return mmq_tile_launch<mmq_tc32_kernel<B200_TYPE_IQ4_XS, false>, Tc32Smem::TOTAL>(a, st); break;
     }
     return B200_ERR_UNSUPPORTED;
 }
@@ -270,10 +344,16 @@ template <bool GROUPED> static int tc32_launch(int type, const Tc32Args & a, cud
 int b200_mmq_tc32(int type, const MmqJob & j, cudaStream_t st) {
     const Tc32Geom g = tc32_geom(j.k, j.ncols);
     Tc32Args a = {};
-    mmq_tile_fill(a, j, (j.k / 32) * type_block_bytes(type));
+    mmq_tile_fill(a, j, (j.k / xf_block_elems(type)) * xf_block_bytes(type));     // Q4_0 / Q5_0 / Q8_0: the repacked rows are as long as the native ones
     a.nks = (int32_t)g.ns;
-    B200_CUDA(b200_launch_pdl(j.map ? quantize_mmq32_kernel<true> : quantize_mmq32_kernel<false>, dim3((unsigned)(j.k / 256), (unsigned)(a.nt * 16)), dim3(256), 0, st,
-                              j.X, j.x_col_stride, j.ncols, j.k_valid, (uint8_t *)j.workspace, g, a.map));
+    if (type == B200_TYPE_IQ4_XS) {
+        if (j.map) return B200_ERR_UNSUPPORTED;
+        B200_CUDA(b200_launch_pdl(quantize_mmq32k_kernel, dim3((unsigned)(j.k / 256), (unsigned)(a.nt * 16)), dim3(256), 0, st,
+                                  j.X, j.x_col_stride, j.ncols, j.k_valid, (uint8_t *)j.workspace, g));
+    } else {
+        B200_CUDA(b200_launch_pdl(j.map ? quantize_mmq32_kernel<true> : quantize_mmq32_kernel<false>, dim3((unsigned)(j.k / 256), (unsigned)(a.nt * 16)), dim3(256), 0, st,
+                                  j.X, j.x_col_stride, j.ncols, j.k_valid, (uint8_t *)j.workspace, g, a.map));
+    }
     b200_count_launch();
     const int rc = j.map ? tc32_launch<true>(type, a, st) : tc32_launch<false>(type, a, st);
     if (a.prof && rc == B200_OK) mmq_prof_report(j.map ? "mmq_tc32 grouped" : "mmq_tc32", type, a, st);

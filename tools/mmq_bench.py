@@ -2,7 +2,7 @@
 """Kernel-level timing of the batched MUL_MAT (b200_mul_mat_q2) on the matmul shapes of the BASELINE models: CUDA events on the
 launching stream, 20 repetitions after 3 warm-ups.
 
-    mmq_bench.py [--cols 512] [--family kquant|block32|q2q3|all] one arm, the shapes at one column count
+    mmq_bench.py [--cols 512] [--family kquant|block32|q2q3|iq4|all]  one arm, the shapes at one column count
     mmq_bench.py --sweep 9,16,32,64,128 --family block32          column sweep on the 8B shapes (where the tensor cores start to win)
     mmq_bench.py --arms [--reps 3] ...                            both arms (tensor cores / column groups through the matvec,
                                                                   B200_MMQ_DISABLE_TC=1) as alternating child processes, the median
@@ -10,9 +10,10 @@ launching stream, 20 repetitions after 3 warm-ups.
 
 q2q3: Q2_K and Q3_K (the wide path's formats) on the Llama-3-8B and Llama-3-70B projection shapes, weights in ggml's native block layout
 (the layout the library keeps for them); their other arm is the wide matvec (b200_mul_mat_vec_wide, one pass per column group).
+iq4: IQ4_NL and IQ4_XS on the same shapes, likewise in native layout, on the int8 kernel (mmq_tc32.cu) against the wide matvec.
 
 Useful TFLOP/s = 2 m k n / time; the share of peak is against the data sheet's dense rate of the pipe the kernel uses (int8 1979 TOPS
-for the block-32 formats, f16 989 TFLOP/s for the K-quants; H100 SXM at 700 W)."""
+for the block-32 and IQ4 formats, f16 989 TFLOP/s for the K-quants; H100 SXM at 700 W)."""
 import argparse
 import json
 import os
@@ -32,11 +33,12 @@ def shapes(G, family):
            ("down 4096x14336 Q8_0", G.Q8_0, 4096, 14336), ("output 128256x4096 Q8_0", G.Q8_0, 128256, 4096),
            ("tinyllama 2048x2048 Q4_0", G.Q4_0, 2048, 2048), ("tinyllama gate/up 5632x2048 Q4_0", G.Q4_0, 5632, 2048), ("tinyllama down 2048x5632 Q4_0", G.Q4_0, 2048, 5632),
            ("qwen2-72b down 8192x29568 Q5_0", G.Q5_0, 8192, 29568), ("qwen2-72b down 8192x29568 Q8_0", G.Q8_0, 8192, 29568)]
-    q23 = [(f"{name} {tn}", t, m, k) for name, m, k in [("8b wq/wo 4096x4096", 4096, 4096), ("8b wk/wv 1024x4096", 1024, 4096), ("8b gate/up 14336x4096", 14336, 4096),
-                                                         ("8b down 4096x14336", 4096, 14336), ("70b wq/wo 8192x8192", 8192, 8192), ("70b wk/wv 1024x8192", 1024, 8192),
-                                                         ("70b gate/up 28672x8192", 28672, 8192), ("70b down 8192x28672", 8192, 28672)]
-           for tn, t in (("Q2_K", G.Q2_K), ("Q3_K", G.Q3_K))]
-    return {"kquant": kq, "block32": b32, "q2q3": q23, "all": kq + b32 + q23}[family]
+    llama = [("8b wq/wo 4096x4096", 4096, 4096), ("8b wk/wv 1024x4096", 1024, 4096), ("8b gate/up 14336x4096", 14336, 4096),
+             ("8b down 4096x14336", 4096, 14336), ("70b wq/wo 8192x8192", 8192, 8192), ("70b wk/wv 1024x8192", 1024, 8192),
+             ("70b gate/up 28672x8192", 28672, 8192), ("70b down 8192x28672", 8192, 28672)]
+    q23 = [(f"{name} {tn}", t, m, k) for name, m, k in llama for tn, t in (("Q2_K", G.Q2_K), ("Q3_K", G.Q3_K))]
+    iq4 = [(f"{name} {tn}", t, m, k) for name, m, k in llama for tn, t in (("IQ4_NL", G.IQ4_NL), ("IQ4_XS", G.IQ4_XS))]
+    return {"kquant": kq, "block32": b32, "q2q3": q23, "iq4": iq4, "all": kq + b32 + q23 + iq4}[family]
 
 
 class NativeWeights:
@@ -64,7 +66,7 @@ def worker(args):
     st = torch.cuda.Stream()
     for name, t, m, k in todo:
         gen = torch.Generator(device="cuda"); gen.manual_seed(1)
-        native = t in (G.Q2_K, G.Q3_K)
+        native = t in (G.Q2_K, G.Q3_K, G.IQ4_NL, G.IQ4_XS)
         W = NativeWeights(b, t, m, k) if native else M.Weights(t, m, k, gen=gen)
         kp = k if native else b.lib.b200_padded_k(t, k)
         rb = W.row_bytes if native else b.row_bytes(t, kp)
@@ -83,7 +85,7 @@ def worker(args):
                     call()
                 e1.record(st); st.synchronize()
             ms = e0.elapsed_time(e1) / reps
-            peak = 1979.0 if t in (G.Q4_0, G.Q5_0, G.Q8_0) else 989.0
+            peak = 1979.0 if t in (G.Q4_0, G.Q5_0, G.Q8_0, G.IQ4_NL, G.IQ4_XS) else 989.0
             tf = 2.0 * m * k * n / ms / 1e9
             out.append({"shape": name, "n_tokens": n, "ms": ms, "tflops_useful": tf, "share_of_pipe_peak": tf / peak, "weight_GBps_per_pass": m * rb / ms / 1e6})
             if args.dump:
@@ -127,7 +129,7 @@ def arms(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--cols", type=int, default=512); ap.add_argument("--sweep", default=""); ap.add_argument("--family", default="all", choices=["kquant", "block32", "q2q3", "all"])
+    ap.add_argument("--cols", type=int, default=512); ap.add_argument("--sweep", default=""); ap.add_argument("--family", default="all", choices=["kquant", "block32", "q2q3", "iq4", "all"])
     ap.add_argument("--arms", action="store_true"); ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--worker", action="store_true"); ap.add_argument("--dump", default="")
     a = ap.parse_args()

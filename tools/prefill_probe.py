@@ -2,7 +2,8 @@
 """Prefill tok/s through the product path (libllama + libggml-b200.so, in-process) on a synthetic GGUF (--config / --ftype,
 default Llama-3-8B Q4_K_M): a 4096-token prompt in 512-token ubatches (BASELINE config 3) and the first 512-token ubatch alone;
 F16 and Q8_0 KV.  B200_MMQ_DISABLE_TC=1 in the environment times the column-group arm of the batched MUL_MAT.
-Q2_K / Q3_K_M files (--ftype) run on the device with GGML_B200_WIDE=1 in the environment; their column-group arm is the wide matvec."""
+Q2_K / Q3_K_M / IQ4_NL / IQ4_XS files (--ftype) run on the device with GGML_B200_WIDE=1 in the environment; their column-group arm is
+the wide matvec."""
 import argparse
 import os
 import subprocess
